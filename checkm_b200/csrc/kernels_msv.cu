@@ -27,7 +27,10 @@ template <int J> __host__ __device__ constexpr int tile_table_bytes() { return s
 template <int J> __host__ __device__ constexpr int tile_block_bytes() { return ssv_block_bytes(J); }
 
 
-template <int J>
+// CHAINED: the tile is one link of a chain (a model of M >= 64 J positions): cell 0 of every row continues the previous
+// link's last cell (bnd_in, null for the first link) and the last cell is handed on (bnd_out, null for the last link).
+// Unchained tiles compile without those loads, stores and register moves in the row loop.
+template <int J, bool CHAINED>
 __device__ __forceinline__ void ssv_rows(const uint8_t *__restrict__ res, int L, uint32_t tile_smem, int lane, uint32_t sel,
                                          const int16_t *bnd_in, int16_t *bnd_out, uint32_t (&u)[J], uint32_t &xE) {
   constexpr int G = J / 4;
@@ -47,7 +50,7 @@ __device__ __forceinline__ void ssv_rows(const uint8_t *__restrict__ res, int L,
 #pragma unroll
     for (int g = G0; g < G; ++g) e[g] = lds128(row + (g - (I8 ? G0 - 1 : 0)) * 512);
     uint32_t bndw = 0;
-    if (bnd_in != nullptr) bndw = (i > 0) ? (uint32_t)(uint16_t)bnd_in[i - 1] : 0u;      // chained tile: cell 0 continues the previous chunk's last cell
+    if (CHAINED && bnd_in != nullptr) bndw = (i > 0) ? (uint32_t)(uint16_t)bnd_in[i - 1] : 0u;
     const uint32_t sh = __shfl_sync(0xffffffffu, u[J - 1], (lane + 31) & 31);
 #pragma unroll
     for (int q = J - 1; q >= 1; --q) {
@@ -58,7 +61,7 @@ __device__ __forceinline__ void ssv_rows(const uint8_t *__restrict__ res, int L,
     u[0] = __viaddmax_s16x2_relu(p0, e[0].x, 0x80008000u);
 #pragma unroll
     for (int q = 0; q < J; q += 2) xE = __vimax3_s16x2(xE, u[q], u[q + 1]);
-    if (bnd_out != nullptr && lane == 31) bnd_out[i] = (int16_t)(u[J - 1] >> 16);
+    if (CHAINED && bnd_out != nullptr && lane == 31) bnd_out[i] = (int16_t)(u[J - 1] >> 16);
   };
   // full blocks of 16 rows, then the tail in groups of 4 (at most 3 padding rows are swept; they score -inf everywhere)
   const int nfull = L >> 4;
@@ -143,9 +146,13 @@ __global__ void __launch_bounds__(SSV_WARPS * 32, 1) ssv_kernel(SsvParams p) {
 #pragma unroll
         for (int q = 0; q < J; ++q) u[q] = 0u;
         uint32_t xE = 0u;
-        const int16_t *bin_ = (nt > 1 && tt > 0) ? ((tt & 1) ? bndA : bndB) : nullptr;
-        int16_t *bout = (nt > 1 && tt + 1 < nt) ? ((tt & 1) ? bndB : bndA) : nullptr;
-        ssv_rows<J>(res, L, tsm, lane, sel, bin_, bout, u, xE);
+        if (nt > 1) {
+          const int16_t *bin_ = (tt > 0) ? ((tt & 1) ? bndA : bndB) : nullptr;
+          int16_t *bout = (tt + 1 < nt) ? ((tt & 1) ? bndB : bndA) : nullptr;
+          ssv_rows<J, true>(res, L, tsm, lane, sel, bin_, bout, u, xE);
+        } else {
+          ssv_rows<J, false>(res, L, tsm, lane, sel, nullptr, nullptr, u, xE);
+        }
         my_cells += (unsigned long long)L * (2 * J);
         // ---- epilogue: does any slot reach the candidate bound? ----
         const uint8_t *meta = smem + tl * TB + tile_table_bytes<J>();

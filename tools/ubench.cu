@@ -58,6 +58,9 @@ __global__ void k(unsigned *out, int iters, unsigned seed) {
         unsigned p0 = __byte_perm(sh, 0, lane ? 0x3210 : 0x1054);
         HR2(a0, p0, v.x)
         x = __vimax3_u16x2(x, a0, a1); x = __vimax3_u16x2(x, a2, a3);
+      } else if (MODE == 9) { // PRMT with the sign-replicating selector the SSV int8 unpack uses
+#define PR(v) asm volatile("prmt.b32 %0, %0, %1, 0x9180;" : "+r"(v) : "r"(d));
+        PR(a0) PR(a1) PR(a2) PR(a3) PR(a4) PR(a5) PR(a6) PR(a7)
       }
     }
   }
@@ -93,6 +96,7 @@ int main() {
     run<6>("SHFL (x4)", 4, threads);
     run<7>("SSV row DPX (1 row = 256 cells)", 1, threads);
     run<8>("SSV row HFMA2 (1 row = 256 cells)", 1, threads);
+    run<9>("PRMT (sign-extend)", 8, threads);
   }
   return 0;
 }
