@@ -58,6 +58,8 @@ static int build_masks(const ckm_models *m, const ckm_seqdb *db, const int32_t *
     } else {
       for (int64_t i = bin_model_offsets[b]; i < bin_model_offsets[b + 1]; ++i) {
         if (model_idx[i] < 0 || model_idx[i] >= ndb) { set_error("model index out of range"); return CKM_EINVAL; }
+        // a model listed twice would be searched once but counted twice in the bin's pairs: refused, as in a shared list
+        if (ma[(size_t)b * ndb + model_idx[i]]) { set_error("duplicate model index in the query list of bin " + std::to_string(b)); return CKM_EINVAL; }
         ma[(size_t)b * ndb + model_idx[i]] = 1;
       }
     }
@@ -354,6 +356,13 @@ struct EnvRunner {
   int nsm;
 };
 static int64_t env_scratch_budget() {
+  // CKM_ENV_SCRATCH_MB (a positive number of MiB, read on every search) replaces the rule below for each engine: a small
+  // budget splits the envelopes of any batch into many waves, a large one keeps them in one.  The waves change no result.
+  if (const char *v = std::getenv("CKM_ENV_SCRATCH_MB")) {
+    char *end = nullptr;
+    const long long mb = std::strtoll(v, &end, 10);
+    if (end != v && *end == '\0' && mb > 0) return (int64_t)std::min<long long>(mb, (long long)1 << 30) * ((int64_t)1 << 20) / (int64_t)sizeof(float);
+  }
   // fixed scratch budget (the cached pool is reused by every later search): 40% of the device shared by the live engines,
   // at most 56 GiB each.  The rest holds each engine's other workspace (for a batch of 32 bins x 5,000 models ~10 GB of
   // Forward/Backward special-state columns and lists), the sequence and model databases, and the caller's own buffers --
@@ -596,7 +605,7 @@ static int do_search(ckm_engine *e, const ckm_models *m, const int32_t *model_id
       // hide under (32-bin batch: domain stage 501 -> 485 ms); with a single wave it is queued after the envelope kernels and takes
       // the SMs as they drain.  CKM_ENS_FIRST=1 / 0 forces one order.
       EnsembleJob *job = nullptr;
-      static const int ens_knob = [] { const char *v = std::getenv("CKM_ENS_FIRST"); return v == nullptr ? -1 : (v[0] == '0' ? 0 : 1); }();
+      const int ens_knob = [] { const char *v = std::getenv("CKM_ENS_FIRST"); return v == nullptr ? -1 : (v[0] == '0' ? 0 : 1); }();
       bool ens_first = (ens_knob == 1);
       if (ens_knob < 0 && !multi_idx.empty()) {
         int64_t tot = 0;

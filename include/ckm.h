@@ -150,7 +150,9 @@ void ckm_seqdb_free(ckm_seqdb *db);
  * given, then by target E-value -- the order hmmsearch writes them. */
 int  ckm_search(ckm_engine *e, const ckm_models *m, const int32_t *model_idx, int32_t nmodels,
                 const ckm_seqdb *db, double E, double domE, ckm_hit **hits_out, int64_t *nhits_out);
-/* same, with per-bin query subsets (lineage_wf: every bin has its own marker HMMs): CSR over bins */
+/* same, with per-bin query subsets (lineage_wf: every bin has its own marker HMMs): CSR over bins.  A bin's rows come in
+ * the order of its own list; an empty list gives the bin no rows.  A model listed twice -- in one bin's list here, or in
+ * model_idx of ckm_search -- is refused with CKM_EINVAL. */
 int  ckm_search_per_bin(ckm_engine *e, const ckm_models *m, const int32_t *model_idx, const int64_t *bin_model_offsets,
                         const ckm_seqdb *db, double E, double domE, ckm_hit **hits_out, int64_t *nhits_out);
 void ckm_hits_free(ckm_hit *hits);
