@@ -18,6 +18,7 @@
 #include "engine.hpp"
 #include "pool.hpp"
 #include "device_utils.cuh"
+#include "ntrows.cuh"
 
 using namespace ckm;
 
@@ -25,10 +26,8 @@ namespace {
 
 constexpr int NT_THREADS = 256;
 constexpr int NT_WARPS = NT_THREADS / 32;
-constexpr int NT_CHUNK = 64;                         // bytes of one lane in one row: one bit each in a 64-bit mask
-constexpr int NT_ROW = 32 * NT_CHUNK;                // 2 KB: what a warp takes at a time
-constexpr int NT_HALO = 16;                          // bytes staged either side of a row (9 before and 1 after are looked at)
-constexpr int NT_STAGE = NT_HALO + NT_ROW + NT_HALO;
+// NT_CHUNK (64 bytes of one lane: one bit each in a 64-bit mask), NT_ROW, NT_HALO (9 bytes before and 1 after a row are
+// looked at) and NT_STAGE: ntrows.cuh
 constexpr int NT_STAGES = 3;                         // rows in flight per warp
 constexpr int NT_DESC_OFF = NT_STAGES * NT_STAGE;    // per-warp shared memory: the stages, their row descriptors, their mbarriers
 constexpr int NT_BAR_OFF = NT_DESC_OFF + NT_STAGES * 16;
@@ -43,10 +42,8 @@ constexpr int NT_CTAS_PER_SM = CKM_NT_CTAS;          // 4: 32 warps x 3 x 2 KB o
 // ahead.  Warps never wait for each other.  A "piece" is the part of one scaffold inside one warp's range.  Contigs closed
 // inside a piece are reported by the kernel; the bases before the first run end of a piece (head) and after its last (tail)
 // come back separately and the host joins tail + head across the cuts (ckm_scaffold_stats below).
-// Piece index = scaffold + warp: along the list one of the two grows at every cut.
-// src: device address the row's copy starts at (16 bytes before the row unless it is the first of its scaffold);
-// info: valid bytes (1..2048) | 16-byte units of the copy << 12 | first row << 30 | last row << 31
-struct NtRow { uint64_t src; uint32_t scaf; uint32_t info; };
+// Piece index = scaffold + warp: along the list one of the two grows at every cut.  The rows (NtRow) and the copies that
+// stage them (nt_issue, nt_wait): ntrows.cuh.
 struct NtPiece { uint32_t head, tail, closed, pad; };              // closed: the piece holds at least one run end
 
 struct NtParams {
@@ -70,27 +67,6 @@ __device__ __forceinline__ uint32_t eq4(uint32_t w, uint32_t pat) {
 __device__ __forceinline__ uint32_t nibble(uint32_t flags) { return (((flags >> 7) * 0x01020408u) >> 24) & 0xFu; }
 // sum of the four bytes of x (the sum must stay below 256)
 __device__ __forceinline__ uint32_t hsum4(uint32_t x) { return (x * 0x01010101u) >> 24; }
-
-// lane 0: hand a stage to the copy engine.  Every value loaded from the stage has been used by now, so the loads are done.
-__device__ __forceinline__ void nt_issue(const NtRow d, uint32_t stage, uint32_t desc, uint32_t bar) {
-  asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(desc), "r"((uint32_t)d.src), "r"((uint32_t)(d.src >> 32)), "r"(d.scaf), "r"(d.info) : "memory");
-  const uint32_t bytes = ((d.info >> 12) & 0xFFu) * 16u;
-  fence_proxy_async();
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(stage + (((d.info >> 30) & 1u) ? (uint32_t)NT_HALO : 0u)),
-               "l"(d.src), "r"(bytes), "r"(bar) : "memory");
-}
-__device__ __forceinline__ void nt_wait(uint32_t bar, uint32_t parity) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "NT_WAIT:\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-      "@p bra NT_DONE;\n"
-      "bra NT_WAIT;\n"
-      "NT_DONE:\n"
-      "}\n" ::"r"(bar), "r"(parity) : "memory");
-}
 
 __device__ __forceinline__ void nt_emit(const NtParams &p, uint32_t scaf, uint32_t len) {
   if (len == 0) return;
@@ -344,16 +320,7 @@ int ckm_scaffold_stats(ckm_engine *e, const uint8_t *bytes, int64_t nbytes, cons
   DevBuf dbytes;
   { int rc0 = dbytes.alloc((size_t)nbytes + 64); if (rc0) return rc0; }
   std::vector<NtRow> rows;
-  rows.reserve((size_t)(nbytes / NT_ROW) + nscaf);
-  for (int32_t s = 0; s < nscaf; ++s)
-    for (int64_t off = 0; off < lens[s]; off += NT_ROW) {
-      const int64_t n = std::min<int64_t>(NT_ROW, lens[s] - off);
-      const bool first = off == 0, last = off + NT_ROW >= lens[s];
-      const int64_t left = first ? 0 : NT_HALO, copy = left + (n + 63) / 64 * 64 + (last ? 0 : NT_HALO);
-      NtRow r; r.src = (uint64_t)(uintptr_t)(dbytes.as<uint8_t>() + starts[s] + off - left); r.scaf = (uint32_t)s;
-      r.info = (uint32_t)n | ((uint32_t)(copy / 16) << 12) | (first ? 1u << 30 : 0u) | (last ? 1u << 31 : 0u);
-      rows.push_back(r);
-    }
+  nt_build_rows(dbytes.as<uint8_t>(), starts, lens, nscaf, nbytes, rows);
   const int64_t nrows = (int64_t)rows.size();
   std::memset(stats_out, 0, sizeof(int64_t) * 8 * nscaf);
   if (nrows == 0) return CKM_OK;

@@ -185,6 +185,21 @@ class Engine:
             check(rc)
             return stats, cscaf[:found.value].astype(np.int64), clen[:found.value].astype(np.int64), float(ms.value)
 
+    def kmer_counts(self, data, starts, lens, k=4):
+        """Canonical k-mer counts of sequences laid out as `seqio.scan_nt_fasta` returns them (ckm_kmer_counts): n x C
+        uint32, C = 2, 10, 32, 136 for k = 1..4, columns in GenomicSignatures.canonicalKmerOrder() order; and the scan
+        kernel's duration in ms."""
+        n = len(lens)
+        ncols = {1: 2, 2: 10, 3: 32, 4: 136}.get(int(k), 1)
+        counts = np.zeros((n, ncols), dtype=np.uint32)
+        data = np.ascontiguousarray(data, dtype=np.uint8)
+        starts = np.ascontiguousarray(starts, dtype=np.int64)
+        lens = np.ascontiguousarray(lens, dtype=np.int64)
+        ms = C.c_float()
+        check(_lib.lib().ckm_kmer_counts(self._h, data.ctypes.data, data.size, starts.ctypes.data, lens.ctypes.data, n, int(k),
+                                         counts.ctypes.data, C.byref(ms)))
+        return counts, float(ms.value)
+
     def close(self):
         if self._h:
             _lib.lib().ckm_destroy(self._h)

@@ -269,6 +269,23 @@ int  ckm_scaffold_stats(ckm_engine *e, const uint8_t *bytes, int64_t nbytes, con
                         int32_t nscaf, int64_t *stats_out, uint32_t *contig_scaffold_out, uint32_t *contig_len_out,
                         int64_t contig_cap, int64_t *ncontigs_out, float *kernel_ms_out);
 
+/* ---- genomic signatures (`checkm tetra`; checkm/genomicSignatures.py:44-84,131-149): canonical k-mer counts of every
+ * sequence as one byte scan on the device, and the profile lines written from them on the host. ---- */
+/* counts_out: nseq x C uint32, C = 2, 10, 32, 136 for k = 1..4, the columns in the order of ckm_kmer_columns.  Every window of
+ * k bytes that is all A/C/G/T (either case; U is not T here) adds one to the column of the smaller of the k-mer and its
+ * reverse complement; every other window is skipped.  Same layout and checks as ckm_scaffold_stats; k outside 1..4 ->
+ * CKM_EINVAL.  kernel_ms_out (optional): duration of the scan kernel by CUDA events. */
+int  ckm_kmer_counts(ckm_engine *e, const uint8_t *bytes, int64_t nbytes, const int64_t *starts, const int64_t *lens,
+                     int32_t nseq, int32_t k, uint32_t *counts_out, float *kernel_ms_out);
+/* host only: the C column names of k, k characters each, written back to back into out (k * C bytes, no terminator) */
+int  ckm_kmer_columns(int32_t k, char *out);
+/* host only: one line per sequence, "id\tv1\t...\tvC\n" with v = count / (sum of the counts) in IEEE double, printed as
+ * Python prints an np.float64 (shortest round-trip digits; 0.0001 but 1e-05); a sequence without a counted window prints
+ * nan in every column.  Ids: ids[id_offsets[s] .. id_offsets[s+1]).  *out_len: the bytes written, or, with CKM_ECAPACITY,
+ * the bytes needed. */
+int  ckm_format_kmer_profiles(const uint32_t *counts, int32_t nseq, int32_t k, const char *ids, const int64_t *id_offsets,
+                              char *out, int64_t out_cap, int64_t *out_len);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1,4 +1,5 @@
-// ubench.cu -- issue-rate microbenchmarks for the instructions the SSV kernel is built from.
+// ubench.cu -- issue-rate microbenchmarks for the instructions the SSV kernel is built from, and for the shared-memory
+// atomics of the k-mer histogram (kmers.cu).
 //   nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o tools/ubench tools/ubench.cu
 #include <cstdio>
 #include <cuda_runtime.h>
@@ -61,6 +62,15 @@ __global__ void k(unsigned *out, int iters, unsigned seed) {
       } else if (MODE == 9) { // PRMT with the sign-replicating selector the SSV int8 unpack uses
 #define PR(v) asm volatile("prmt.b32 %0, %0, %1, 0x9180;" : "+r"(v) : "r"(d));
         PR(a0) PR(a1) PR(a2) PR(a3) PR(a4) PR(a5) PR(a6) PR(a7)
+      } else if (MODE >= 10 && MODE <= 13) { // shared-memory add into a per-warp 256-word histogram (+1 IMAD each):
+        // 10 red.add, random bins; 11 red.add, one bin for the whole warp (homopolymer); 12 red.add, two bins
+        // (dinucleotide repeat); 13 atom.add (result used), random bins
+        const unsigned hist = (unsigned)__cvta_generic_to_shared(sm) + (threadIdx.x >> 5) * 1024u;
+#define HB(v) { v = v * 1664525u + 1013904223u; \
+                const unsigned bin = MODE == 11 ? (v & 0u) : MODE == 12 ? (lane & 1u) * 37u + (v & 0u) : v >> 24; \
+                if (MODE == 13) { unsigned o; asm volatile("atom.shared.add.u32 %0, [%1], 1;" : "=r"(o) : "r"(hist + bin * 4u) : "memory"); x += o; } \
+                else asm volatile("red.shared.add.u32 [%0], 1;" :: "r"(hist + bin * 4u) : "memory"); }
+        HB(a0) HB(a1) HB(a2) HB(a3)
       }
     }
   }
@@ -97,6 +107,10 @@ int main() {
     run<7>("SSV row DPX (1 row = 256 cells)", 1, threads);
     run<8>("SSV row HFMA2 (1 row = 256 cells)", 1, threads);
     run<9>("PRMT (sign-extend)", 8, threads);
+    run<10>("red.shared.add random bins (x4)", 4, threads);
+    run<11>("red.shared.add one bin/warp (x4)", 4, threads);
+    run<12>("red.shared.add two bins/warp (x4)", 4, threads);
+    run<13>("atom.shared.add random bins (x4)", 4, threads);
   }
   return 0;
 }
