@@ -69,7 +69,7 @@ SYMBOLS = ["ckm_init", "ckm_destroy", "ckm_last_error", "ckm_version", "ckm_devi
            "ckm_search", "ckm_search_per_bin", "ckm_hits_free", "ckm_align", "ckm_last_stats", "ckm_msv_scores",
            "ckm_filter_scores", "ckm_viterbi_scores", "ckm_write_domtblout", "ckm_reduce", "ckm_genome_check", "ckm_free", "ckm_allgather_qa", "ckm_nccl_unique_id",
            "ckm_nccl_comm_init", "ckm_nccl_comm_destroy", "ckm_fasta_scan_nt", "ckm_scaffold_stats",
-           "ckm_kmer_counts", "ckm_kmer_columns", "ckm_format_kmer_profiles"]
+           "ckm_kmer_counts", "ckm_kmer_columns", "ckm_format_kmer_profiles", "ckm_merge_pairs", "ckm_format_merger_rows"]
 
 _lib = None
 
@@ -104,6 +104,8 @@ def lib():
     L.ckm_kmer_counts.argtypes = [vp, vp, i64, vp, vp, i32, i32, vp, C.POINTER(C.c_float)]
     L.ckm_kmer_columns.argtypes = [i32, vp]
     L.ckm_format_kmer_profiles.argtypes = [vp, i32, i32, vp, vp, vp, i64, C.POINTER(i64)]
+    L.ckm_merge_pairs.argtypes = [vp, vp, i32, i32, vp, dbl, dbl, dbl, dbl, vp, i64, C.POINTER(i64), C.POINTER(C.c_float)]
+    L.ckm_format_merger_rows.argtypes = [vp, vp, i32, vp, vp, vp, vp, i64, vp, i64, C.POINTER(i64)]
     L.ckm_seqdb_create.argtypes = [vp, vp, vp, i32, vp, i32, C.POINTER(vp)]
     L.ckm_seqdb_free.argtypes = [vp]
     L.ckm_seqdb_free.restype = None

@@ -10,6 +10,7 @@ ALPHABET = "ACDEFGHIKLMNPQRSTVWY-BJZOUX*~"
 HIT_DTYPE = np.dtype([(n, {C.c_int32: np.int32, C.c_float: np.float32, C.c_double: np.float64}[t]) for n, t in Hit._fields_],
                      align=True)
 assert HIT_DTYPE.itemsize == C.sizeof(Hit)
+MERGE_PAIR_DTYPE = np.dtype([('i', np.int32), ('j', np.int32), ('p', np.int32), ('s', np.int32)])   # ckm_merge_pair
 
 
 def digitize(text):
@@ -199,6 +200,30 @@ class Engine:
         check(_lib.lib().ckm_kmer_counts(self._h, data.ctypes.data, data.size, starts.ctypes.data, lens.ctypes.data, n, int(k),
                                          counts.ctypes.data, C.byref(ms)))
         return counts, float(ms.value)
+
+    def merge_pairs(self, counts, n_markers, min_delta_comp, max_delta_cont, min_merged_comp, max_merged_cont, capacity=None):
+        """The bin pairs `checkm merge` reports (ckm_merge_pairs).  counts: nbins x nmarkers copy numbers, one row per bin
+        in sorted() id order; n_markers: numMarkers() of each bin's marker set.  Returns the kept pairs as a
+        MERGE_PAIR_DTYPE array (i ascending, then j) and the kernels' duration in ms.  When more pairs pass than `capacity`
+        (default: 16 per bin) the call is repeated with room for exactly the number that came back."""
+        counts = np.ascontiguousarray(counts, dtype=np.int32)
+        n_markers = np.ascontiguousarray(n_markers, dtype=np.int32)
+        if counts.ndim != 2 or n_markers.shape != (counts.shape[0],):
+            raise ValueError("merge_pairs: counts must be nbins x nmarkers and n_markers hold one value per bin")
+        nb, nm = counts.shape
+        cap = min(nb * (nb - 1) // 2, 16 * nb + 1024) if capacity is None else int(capacity)
+        while True:
+            out = np.empty(cap, dtype=MERGE_PAIR_DTYPE)
+            found, ms = C.c_int64(), C.c_float()
+            rc = _lib.lib().ckm_merge_pairs(self._h, counts.ctypes.data if counts.size else None, nb, nm,
+                                            n_markers.ctypes.data if nb else None, float(min_delta_comp), float(max_delta_cont),
+                                            float(min_merged_comp), float(max_merged_cont), out.ctypes.data if cap else None,
+                                            cap, C.byref(found), C.byref(ms))
+            if rc == 8 and found.value > cap:          # CKM_ECAPACITY: the count needed came back
+                cap = found.value
+                continue
+            check(rc)
+            return out[:found.value], float(ms.value)
 
     def close(self):
         if self._h:

@@ -286,6 +286,25 @@ int  ckm_kmer_columns(int32_t k, char *out);
 int  ckm_format_kmer_profiles(const uint32_t *counts, int32_t nseq, int32_t k, const char *ids, const int64_t *id_offsets,
                               char *out, int64_t out_cap, int64_t *out_len);
 
+/* ---- bin mergers (`checkm merge`; checkm/merger.py:34-110): every pair of bins scored in one device pass, and the
+ * merger.tsv rows written from the passing pairs on the host.  The arithmetic is stated in csrc/merge.cu. ---- */
+typedef struct { int32_t i, j, p, s; } ckm_merge_pair;   /* bins i < j, markers present p and hits s of the merged pair */
+/* counts: nbins x nmarkers int32 copy numbers (>= 0; each bin's sum below 2^30), one row per bin in sorted() id order,
+ * one column per marker of the shared marker union; n_markers: per bin, numMarkers() of its marker set (>= 1; the merged
+ * pair is scored with bin j's).  A pair is kept iff comp >= min_merged_comp, cont < max_merged_cont,
+ * comp - max(comp_i, comp_j) >= min_delta_comp and cont - max(cont_i, cont_j) < max_delta_cont, in float64.
+ * pairs_out: the kept pairs, i ascending then j ascending.  *npairs_out: the number kept; with CKM_ECAPACITY (more than
+ * pair_cap) the number needed, and nothing is written.  kernel_ms_out (optional): the device kernels' time by CUDA events. */
+int  ckm_merge_pairs(ckm_engine *e, const int32_t *counts, int32_t nbins, int32_t nmarkers, const int32_t *n_markers,
+                     double min_delta_comp, double max_delta_cont, double min_merged_comp, double max_merged_cont,
+                     ckm_merge_pair *pairs_out, int64_t pair_cap, int64_t *npairs_out, float *kernel_ms_out);
+/* host only: one merger.tsv row per pair, "id_i\tid_j" then the nine values of merger.py:101-106 as "%.2f", each
+ * computed from p, s and n_markers of the bins as the reference does.  Ids: ids[id_offsets[b] .. id_offsets[b+1]).
+ * *out_len: the bytes written, or, with CKM_ECAPACITY, the bytes needed. */
+int  ckm_format_merger_rows(const char *ids, const int64_t *id_offsets, int32_t nbins, const int32_t *p, const int32_t *s,
+                            const int32_t *n_markers, const ckm_merge_pair *pairs, int64_t npairs, char *out, int64_t out_cap,
+                            int64_t *out_len);
+
 #ifdef __cplusplus
 }
 #endif

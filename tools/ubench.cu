@@ -1,5 +1,5 @@
 // ubench.cu -- issue-rate microbenchmarks for the instructions the SSV kernel is built from, and for the shared-memory
-// atomics of the k-mer histogram (kmers.cu).
+// atomics of the k-mer histogram (kmers.cu), and for the AND + POPC pair of the merge Gram kernel (merge.cu).
 //   nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o tools/ubench tools/ubench.cu
 #include <cstdio>
 #include <cuda_runtime.h>
@@ -71,6 +71,9 @@ __global__ void k(unsigned *out, int iters, unsigned seed) {
                 if (MODE == 13) { unsigned o; asm volatile("atom.shared.add.u32 %0, [%1], 1;" : "=r"(o) : "r"(hist + bin * 4u) : "memory"); x += o; } \
                 else asm volatile("red.shared.add.u32 [%0], 1;" :: "r"(hist + bin * 4u) : "memory"); }
         HB(a0) HB(a1) HB(a2) HB(a3)
+      } else if (MODE == 14) { // POPC of (a & d), accumulated: the inner step of merge_gram_kernel, 8 independent chains
+#define PC(v) v += __popc(v & d);
+        PC(a0) PC(a1) PC(a2) PC(a3) PC(a4) PC(a5) PC(a6) PC(a7)
       }
     }
   }
@@ -111,6 +114,7 @@ int main() {
     run<11>("red.shared.add one bin/warp (x4)", 4, threads);
     run<12>("red.shared.add two bins/warp (x4)", 4, threads);
     run<13>("atom.shared.add random bins (x4)", 4, threads);
+    run<14>("POPC(a & b) + IADD (x8; POPC counted)", 8, threads);
   }
   return 0;
 }
