@@ -62,6 +62,10 @@ class ReduceMeta(C.Structure):
                 ("bin_set_off", C.c_void_p), ("set_marker_off", C.c_void_p), ("set_marker_idx", C.c_void_p)]
 
 
+class BamFilter(C.Structure):
+    _fields_ = [("all_reads", C.c_int32), ("min_qc", C.c_int32), ("min_align", C.c_double), ("max_edit", C.c_double)]
+
+
 # every symbol include/ckm.h declares (tests/test_abi.py checks the .so exports each one)
 SYMBOLS = ["ckm_init", "ckm_destroy", "ckm_last_error", "ckm_version", "ckm_device_name",
            "ckm_models_load", "ckm_models_count", "ckm_models_info", "ckm_models_find", "ckm_models_select",
@@ -69,7 +73,8 @@ SYMBOLS = ["ckm_init", "ckm_destroy", "ckm_last_error", "ckm_version", "ckm_devi
            "ckm_search", "ckm_search_per_bin", "ckm_hits_free", "ckm_align", "ckm_last_stats", "ckm_msv_scores",
            "ckm_filter_scores", "ckm_viterbi_scores", "ckm_write_domtblout", "ckm_reduce", "ckm_genome_check", "ckm_free", "ckm_allgather_qa", "ckm_nccl_unique_id",
            "ckm_nccl_comm_init", "ckm_nccl_comm_destroy", "ckm_fasta_scan_nt", "ckm_scaffold_stats",
-           "ckm_kmer_counts", "ckm_kmer_columns", "ckm_format_kmer_profiles", "ckm_merge_pairs", "ckm_format_merger_rows"]
+           "ckm_kmer_counts", "ckm_kmer_columns", "ckm_format_kmer_profiles", "ckm_merge_pairs", "ckm_format_merger_rows",
+           "ckm_bgzf_blocks", "ckm_bgzf_inflate", "ckm_bam_coverage"]
 
 _lib = None
 
@@ -106,6 +111,9 @@ def lib():
     L.ckm_format_kmer_profiles.argtypes = [vp, i32, i32, vp, vp, vp, i64, C.POINTER(i64)]
     L.ckm_merge_pairs.argtypes = [vp, vp, i32, i32, vp, dbl, dbl, dbl, dbl, vp, i64, C.POINTER(i64), C.POINTER(C.c_float)]
     L.ckm_format_merger_rows.argtypes = [vp, vp, i32, vp, vp, vp, vp, i64, vp, i64, C.POINTER(i64)]
+    L.ckm_bgzf_blocks.argtypes = [vp, i64, i64, vp, i64, C.POINTER(i64), C.POINTER(i64)]
+    L.ckm_bgzf_inflate.argtypes = [vp, vp, i64, i64, vp, i64, vp, i64, C.POINTER(i64), C.POINTER(C.c_float)]
+    L.ckm_bam_coverage.argtypes = [vp, vp, i64, i64, vp, i64, vp, vp, i64, i32, C.POINTER(BamFilter), vp, vp, C.POINTER(i64)]
     L.ckm_seqdb_create.argtypes = [vp, vp, vp, i32, vp, i32, C.POINTER(vp)]
     L.ckm_seqdb_free.argtypes = [vp]
     L.ckm_seqdb_free.restype = None

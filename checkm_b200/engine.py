@@ -225,6 +225,38 @@ class Engine:
             check(rc)
             return out[:found.value], float(ms.value)
 
+    def bgzf_inflate(self, comp, blocks, comp_base=0):
+        """The payloads of BGZF `blocks` (a bam.BLOCK_DTYPE table of file offsets; comp[0] is the byte at file offset
+        comp_base) inflated back to back on the device (ckm_bgzf_inflate), and the inflate kernel's duration in ms."""
+        comp = np.ascontiguousarray(np.frombuffer(comp, dtype=np.uint8) if not isinstance(comp, np.ndarray) else comp)
+        blocks = np.ascontiguousarray(blocks)
+        total = int(blocks['isize'].sum())
+        out = np.empty(max(total, 1), dtype=np.uint8)
+        ms = C.c_float()
+        check(_lib.lib().ckm_bgzf_inflate(self._h, comp.ctypes.data if comp.size else None, int(comp_base), comp.size,
+                                          blocks.ctypes.data if len(blocks) else None, len(blocks), out.ctypes.data, out.size,
+                                          None, C.byref(ms)))
+        return out[:total], float(ms.value)
+
+    def bam_coverage(self, comp, blocks, seg_start, seg_end, n_ref, counters, comp_base=0, all_reads=False, min_qc=15,
+                     min_align=0.98, max_edit=0.02):
+        """One batch of a BAM (ckm_bam_coverage): blocks inflated, the segments walked, the nine counters of every
+        reference added to `counters` (n_ref x 9 int64).  Returns the inflate and scan kernels' durations in ms."""
+        comp = np.ascontiguousarray(np.frombuffer(comp, dtype=np.uint8) if not isinstance(comp, np.ndarray) else comp)
+        blocks = np.ascontiguousarray(blocks)
+        seg_start = np.ascontiguousarray(seg_start, dtype=np.int64)
+        seg_end = np.ascontiguousarray(seg_end, dtype=np.int64)
+        if counters.dtype != np.int64 or counters.shape != (n_ref, 9) or not counters.flags.c_contiguous:
+            raise ValueError("bam_coverage: counters must be a C-contiguous n_ref x 9 int64 array")
+        filt = _lib.BamFilter(int(bool(all_reads)), int(min_qc), float(min_align), float(max_edit))
+        ms = (C.c_float * 2)()
+        err = C.c_int64()
+        check(_lib.lib().ckm_bam_coverage(self._h, comp.ctypes.data if comp.size else None, int(comp_base), comp.size,
+                                          blocks.ctypes.data if len(blocks) else None, len(blocks), seg_start.ctypes.data,
+                                          seg_end.ctypes.data, len(seg_start), int(n_ref), C.byref(filt),
+                                          counters.ctypes.data if n_ref else None, ms, C.byref(err)))
+        return float(ms[0]), float(ms[1])
+
     def close(self):
         if self._h:
             _lib.lib().ckm_destroy(self._h)

@@ -453,7 +453,7 @@ class ResultsParser(object):
         oldStdOut = reassignStdOut(outFile)
         coverageBinProfiles = None
         if coverageFile:
-            from checkm.coverage import Coverage        # BAM coverage stays CheckM's (out of the hot path)
+            from .coverage import Coverage
             coverageBinProfiles = Coverage(1).binProfiles(coverageFile)
         self._device_counts(binIdToBinMarkerSets, bIndividualMarkers)
         prettyTableFormats = [1, 2, 3, 9]

@@ -305,6 +305,40 @@ int  ckm_format_merger_rows(const char *ids, const int64_t *id_offsets, int32_t 
                             const int32_t *n_markers, const ckm_merge_pair *pairs, int64_t npairs, char *out, int64_t out_cap,
                             int64_t *out_len);
 
+/* ---- read coverage (`checkm coverage`; checkm/coverage.py:57-287): BGZF blocks inflated and BAM records walked and
+ * classified on the device, nine int64 counters per reference.  The kernels and the anchor argument are described in
+ * csrc/bam.cu. ---- */
+typedef struct { int64_t coffset; int32_t clen; int32_t isize; } ckm_bgzf_block;   /* file offset, bytes (BSIZE + 1), ISIZE */
+/* host only: the BGZF blocks of data[0, n), data[0] being the byte at file offset `base`.  Walks the gzip member headers
+ * (1f 8b 08 04, XLEN, the BC subfield with BSIZE) and stops at the last block wholly inside the range, or after `cap`
+ * blocks, so that a file can be walked in pieces: *consumed_out is the number of bytes the returned blocks cover.  A
+ * header that is not BGZF gives CKM_EFORMAT with its file offset in the message (*consumed_out: its offset in data). */
+int  ckm_bgzf_blocks(const uint8_t *data, int64_t n, int64_t base, ckm_bgzf_block *blocks_out, int64_t cap,
+                     int64_t *nblocks_out, int64_t *consumed_out);
+/* The payloads of `blocks` (file offsets; comp[0] is the byte at file offset comp_base) inflated back to back into out
+ * (the sum of ISIZE bytes).  Every block's CRC32 and ISIZE are checked; a malformed block gives CKM_EFORMAT naming its
+ * file offset, and *bad_block_out (optional) its index.  kernel_ms_out (optional): the inflate kernel by CUDA events. */
+int  ckm_bgzf_inflate(ckm_engine *e, const uint8_t *comp, int64_t comp_base, int64_t comp_len, const ckm_bgzf_block *blocks,
+                      int64_t nblocks, uint8_t *out, int64_t out_cap, int64_t *bad_block_out, float *kernel_ms_out);
+typedef struct {
+  int32_t all_reads;     /* bAllReads: count reads that are not properly paired        */
+  int32_t min_qc;        /* minQC: reads with mapping quality below it fail QC         */
+  double  min_align;     /* minAlignPer: query_alignment_length >= min_align * l_seq   */
+  double  max_edit;      /* maxEditDistPer: NM <= max_edit * l_seq                     */
+} ckm_bam_filter;
+/* One batch of a coordinate-sorted BAM: the blocks are inflated into one stream (block b at U[b], U the exclusive prefix
+ * sum of ISIZE over the batch) and every segment [seg_start[s], seg_end[s]) of that stream is walked record by record.
+ * Each segment must start on a record and its walk must end exactly at seg_end; the walk of the last segment also stops at
+ * the first record with refID -1.  counters (n_ref x 9 int64, added to): reads, duplicates, secondary or supplementary,
+ * failed QC, failed alignment length, failed edit distance, not properly paired, mapped, aligned bases of the mapped reads
+ * (coverage.py:206-230 in that order).  A malformed block or record, a walk that misses its segment end, or a read that
+ * reaches the edit-distance test without an integer NM tag gives CKM_EFORMAT; *err_offset_out is then the bad block's file
+ * offset or the bad record's virtual offset (coffset << 16 | uoffset), and the message names the read for a missing NM.
+ * kernel_ms_out (optional, 2 floats): the inflate and the scan kernel by CUDA events. */
+int  ckm_bam_coverage(ckm_engine *e, const uint8_t *comp, int64_t comp_base, int64_t comp_len, const ckm_bgzf_block *blocks,
+                      int64_t nblocks, const int64_t *seg_start, const int64_t *seg_end, int64_t nseg, int32_t n_ref,
+                      const ckm_bam_filter *filter, int64_t *counters, float *kernel_ms_out, int64_t *err_offset_out);
+
 #ifdef __cplusplus
 }
 #endif
