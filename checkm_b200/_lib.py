@@ -66,6 +66,19 @@ class BamFilter(C.Structure):
     _fields_ = [("all_reads", C.c_int32), ("min_qc", C.c_int32), ("min_align", C.c_double), ("max_edit", C.c_double)]
 
 
+class OutlierIn(C.Structure):
+    _fields_ = [("nseq", C.c_int64), ("nbins", C.c_int32), ("ntables", C.c_int32), ("bin_off", C.c_void_p),
+                ("len", C.c_void_p), ("acgt", C.c_void_p), ("coding", C.c_void_p), ("sig_row", C.c_void_p),
+                ("bin_gc_table", C.c_void_p), ("bin_cd_table", C.c_void_p), ("td_table", C.c_int32), ("pad", C.c_int32),
+                ("table_off", C.c_void_p), ("table_key", C.c_void_p), ("table_lo", C.c_void_p), ("table_hi", C.c_void_p),
+                ("binsig_in", C.c_void_p)]
+
+
+class OutlierOut(C.Structure):
+    _fields_ = [("bin_means", C.c_void_p), ("bin_sig", C.c_void_p), ("seq_values", C.c_void_p), ("seq_mask", C.c_void_p),
+                ("kernel_ms", C.c_float * 3)]
+
+
 # every symbol include/ckm.h declares (tests/test_abi.py checks the .so exports each one)
 SYMBOLS = ["ckm_init", "ckm_destroy", "ckm_last_error", "ckm_version", "ckm_device_name",
            "ckm_models_load", "ckm_models_count", "ckm_models_info", "ckm_models_find", "ckm_models_select",
@@ -74,7 +87,8 @@ SYMBOLS = ["ckm_init", "ckm_destroy", "ckm_last_error", "ckm_version", "ckm_devi
            "ckm_filter_scores", "ckm_viterbi_scores", "ckm_write_domtblout", "ckm_reduce", "ckm_genome_check", "ckm_free", "ckm_allgather_qa", "ckm_nccl_unique_id",
            "ckm_nccl_comm_init", "ckm_nccl_comm_destroy", "ckm_fasta_scan_nt", "ckm_scaffold_stats",
            "ckm_kmer_counts", "ckm_kmer_columns", "ckm_format_kmer_profiles", "ckm_merge_pairs", "ckm_format_merger_rows",
-           "ckm_bgzf_blocks", "ckm_bgzf_inflate", "ckm_bam_coverage"]
+           "ckm_bgzf_blocks", "ckm_bgzf_inflate", "ckm_bam_coverage",
+           "ckm_parse_kmer_profiles", "ckm_sigs_create", "ckm_sigs_free", "ckm_outlier_scores"]
 
 _lib = None
 
@@ -111,6 +125,11 @@ def lib():
     L.ckm_format_kmer_profiles.argtypes = [vp, i32, i32, vp, vp, vp, i64, C.POINTER(i64)]
     L.ckm_merge_pairs.argtypes = [vp, vp, i32, i32, vp, dbl, dbl, dbl, dbl, vp, i64, C.POINTER(i64), C.POINTER(C.c_float)]
     L.ckm_format_merger_rows.argtypes = [vp, vp, i32, vp, vp, vp, vp, i64, vp, i64, C.POINTER(i64)]
+    L.ckm_parse_kmer_profiles.argtypes = [C.c_char_p, i64, i32, i32, vp, vp, vp, i64, C.POINTER(i64)]
+    L.ckm_sigs_create.argtypes = [vp, vp, i64, C.POINTER(vp)]
+    L.ckm_sigs_free.argtypes = [vp]
+    L.ckm_sigs_free.restype = None
+    L.ckm_outlier_scores.argtypes = [vp, vp, C.POINTER(OutlierIn), C.POINTER(OutlierOut)]
     L.ckm_bgzf_blocks.argtypes = [vp, i64, i64, vp, i64, C.POINTER(i64), C.POINTER(i64)]
     L.ckm_bgzf_inflate.argtypes = [vp, vp, i64, i64, vp, i64, vp, i64, C.POINTER(i64), C.POINTER(C.c_float)]
     L.ckm_bam_coverage.argtypes = [vp, vp, i64, i64, vp, i64, vp, vp, i64, i32, C.POINTER(BamFilter), vp, vp, C.POINTER(i64)]

@@ -1,12 +1,15 @@
 """Path and stdout helpers the hot-path classes call (behaviour of the same-named functions of checkm/common.py: same log
 messages, same exit codes).  When CheckM itself is importable its own helpers are used, so a drop-in shares one copy."""
+import ast
 import logging
 import os
 import sys
 
+import numpy as np
+
 try:                                              # inside a CheckM install: CheckM's own helpers
     from checkm.common import (checkFileExists, checkDirExists, makeSurePathExists, binIdFromFilename,       # noqa: F401
-                               getBinIdsFromOutDir, reassignStdOut, restoreStdOut)
+                               getBinIdsFromOutDir, reassignStdOut, restoreStdOut, readDistribution, findNearest)
 except Exception:                                 # stand-alone
     def _fatal(message):
         logging.getLogger('timestamp').error(message + '\n')
@@ -16,6 +19,18 @@ except Exception:                                 # stand-alone
         if os.path.exists(inputFile):
             return
         _fatal('Input file does not exists: ' + inputFile)
+
+    def readDistribution(prefix):
+        """The dictionary literal of <data root>/distributions/<prefix>.txt (common.py:46-55)."""
+        from .defaultValues import DefaultValues
+        distFile = os.path.join(DefaultValues.DISTRIBUTION_DIR, prefix + '.txt')
+        checkFileExists(distFile)
+        with open(distFile, 'r') as f:
+            return ast.literal_eval(f.read())
+
+    def findNearest(array, value):
+        """The element of array nearest to value; of two equally near ones the first (common.py:58-62)."""
+        return array[(np.abs(np.array(array) - value)).argmin()]
 
     def checkDirExists(inputDir):
         if os.path.exists(inputDir):

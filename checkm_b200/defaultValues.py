@@ -34,6 +34,7 @@ class DefaultValues(object):
     SELECTED_MARKER_SETS = os.path.join(CHECKM_DATA_DIR, 'selected_marker_sets.tsv')
     TAXON_MARKER_SETS = os.path.join(CHECKM_DATA_DIR, 'taxon_marker_sets.tsv')
     GENOME_TREE_DIR = os.path.join(CHECKM_DATA_DIR, 'genome_tree')                      # defaultValues.py:60-70
+    DISTRIBUTION_DIR = os.path.join(CHECKM_DATA_DIR, 'distributions')                   # defaultValues.py:71
     GENOME_TREE_METADATA = 'genome_tree.metadata.tsv'
     GENOME_TREE_MISSING_DUPLICATE = 'missing_duplicate_genes_50.tsv'
     PPLACER_TREE_OUT = 'concatenated.tre'                                               # defaultValues.py:89
@@ -63,3 +64,4 @@ class DefaultValues(object):
         cls.SELECTED_MARKER_SETS = os.path.join(root, 'selected_marker_sets.tsv')
         cls.TAXON_MARKER_SETS = os.path.join(root, 'taxon_marker_sets.tsv')
         cls.GENOME_TREE_DIR = os.path.join(root, 'genome_tree')
+        cls.DISTRIBUTION_DIR = os.path.join(root, 'distributions')

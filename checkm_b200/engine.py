@@ -21,6 +21,23 @@ def digitize(text):
     return out
 
 
+class Signatures:
+    """A profile matrix (n x 136 float64) resident on the device for the outlier calls of one run (ckm_sigs_create)."""
+
+    def __init__(self, engine, values):
+        values = np.ascontiguousarray(values, dtype=np.float64)
+        if values.ndim != 2 or values.shape[1] != 136 or values.shape[0] < 1:
+            raise ValueError("Signatures: values must be n x 136 with n >= 1")
+        self.n = values.shape[0]
+        self._h = C.c_void_p()
+        check(_lib.lib().ckm_sigs_create(engine._h, values.ctypes.data, self.n, C.byref(self._h)))
+
+    def close(self):
+        if self._h:
+            _lib.lib().ckm_sigs_free(self._h)
+            self._h = C.c_void_p()
+
+
 class Models:
     def __init__(self, engine, path):
         self.engine = engine
@@ -224,6 +241,41 @@ class Engine:
                 continue
             check(rc)
             return out[:found.value], float(ms.value)
+
+    def signatures(self, values):
+        return Signatures(self, values)
+
+    def outlier_scores(self, sigs, bin_off, lens, acgt, coding, sig_row, bin_gc_table, bin_cd_table, td_table, table_off,
+                       table_key, table_lo, table_hi, binsig_in=None, want_binsig=False):
+        """Every sequence of a batch of bins scored against its bin (ckm_outlier_scores; the arguments are the fields of
+        ckm_outlier_in).  Returns bin_means (nbins x 3: meanGC, meanCD, meanTD), the bins' signatures (nbins x 136, or None
+        unless want_binsig), seq_values (nseq x 9: GC, deltaGC, CD, deltaCD, TD, GC lower, GC upper, CD lower, TD upper),
+        the outlying mask per sequence (1 GC, 2 CD, 4 TD) and the three kernels' durations in ms."""
+        i64 = lambda a: np.ascontiguousarray(a, dtype=np.int64)       # noqa: E731
+        f64 = lambda a: np.ascontiguousarray(a, dtype=np.float64)     # noqa: E731
+        bin_off, lens, acgt, coding, sig_row, table_off = (i64(a) for a in (bin_off, lens, acgt, coding, sig_row, table_off))
+        bin_gc_table = np.ascontiguousarray(bin_gc_table, dtype=np.int32)
+        bin_cd_table = np.ascontiguousarray(bin_cd_table, dtype=np.int32)
+        table_key, table_lo, table_hi = f64(table_key), f64(table_lo), f64(table_hi)
+        nb, ns, nt = len(bin_off) - 1, len(lens), len(table_off) - 1
+        if (acgt.shape != (ns, 4) or coding.shape != (ns,) or sig_row.shape != (ns,) or bin_gc_table.shape != (nb,) or
+                bin_cd_table.shape != (nb,) or not (table_key.shape == table_lo.shape == table_hi.shape == (int(table_off[-1]),))):
+            raise ValueError("outlier_scores: array shapes do not agree")
+        if binsig_in is not None:
+            binsig_in = f64(binsig_in)
+            if binsig_in.shape != (nb, 136):
+                raise ValueError("outlier_scores: binsig_in must be nbins x 136")
+        means = np.empty((nb, 3), dtype=np.float64)
+        binsig = np.empty((nb, 136), dtype=np.float64) if want_binsig else None
+        values = np.empty((ns, 9), dtype=np.float64)
+        mask = np.empty(ns, dtype=np.uint8)
+        arg = _lib.OutlierIn(ns, nb, nt, bin_off.ctypes.data, lens.ctypes.data, acgt.ctypes.data, coding.ctypes.data,
+                             sig_row.ctypes.data, bin_gc_table.ctypes.data, bin_cd_table.ctypes.data, int(td_table), 0,
+                             table_off.ctypes.data, table_key.ctypes.data, table_lo.ctypes.data, table_hi.ctypes.data,
+                             binsig_in.ctypes.data if binsig_in is not None else None)
+        out = _lib.OutlierOut(means.ctypes.data, binsig.ctypes.data if want_binsig else None, values.ctypes.data, mask.ctypes.data)
+        check(_lib.lib().ckm_outlier_scores(self._h, sigs._h, C.byref(arg), C.byref(out)))
+        return means, binsig, values, mask, tuple(float(v) for v in out.kernel_ms)
 
     def bgzf_inflate(self, comp, blocks, comp_base=0):
         """The payloads of BGZF `blocks` (a bam.BLOCK_DTYPE table of file offsets; comp[0] is the byte at file offset

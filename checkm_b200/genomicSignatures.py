@@ -50,6 +50,22 @@ def format_profiles(counts, ids, K):
     return out.raw[:used.value]
 
 
+def parse_profiles(raw, ncols=136, threads=1):
+    """The profile file's bytes -> the ids of its lines (in file order, repeats included) and their values as an
+    n x ncols float64 matrix, each value what float() makes of its text (ckm_parse_kmer_profiles, up to `threads` host
+    threads)."""
+    cap = raw.count(b'\n') + 1
+    starts = np.empty(cap, dtype=np.int64)
+    id_lens = np.empty(cap, dtype=np.int32)
+    values = np.empty((cap, ncols), dtype=np.float64)
+    found = C.c_int64()
+    _lib.check(_lib.lib().ckm_parse_kmer_profiles(raw, len(raw), ncols, max(1, int(threads or 1)), starts.ctypes.data,
+                                                  id_lens.ctypes.data, values.ctypes.data, cap, C.byref(found)))
+    n = found.value
+    ids = [raw[a:a + k].decode('utf-8', 'replace') for a, k in zip(starts[:n].tolist(), id_lens[:n].tolist())]
+    return ids, values[:n]
+
+
 def _monotonic(data, starts, lens):
     """The layout with starts in increasing order (scan_nt_fasta keeps a repeated id in its first place but with its last
     record's bytes, so starts can go backwards)."""

@@ -305,6 +305,50 @@ int  ckm_format_merger_rows(const char *ids, const int64_t *id_offsets, int32_t 
                             const int32_t *n_markers, const ckm_merge_pair *pairs, int64_t npairs, char *out, int64_t out_cap,
                             int64_t *out_len);
 
+/* ---- sequence outliers (`checkm outliers`; checkm/binTools.py:148-296): every sequence of a batch of bins scored against
+ * its bin's GC, coding density and tetranucleotide signature in one device pass.  The arithmetic, and the order of every
+ * floating-point sum, is stated in csrc/outliers.cu. ---- */
+/* host only (replaces GenomicSignatures.read, genomicSignatures.py:189-200, which binTools.py:236-237 calls once per bin):
+ * the profile file `text` (a header line, then "id\tv1\t...\tvN" per line, N = ncols) in one pass over up to nthreads host
+ * threads.  Row r: id = text[id_start_out[r] .. + id_len_out[r]), values_out[r * ncols ..] = the correctly rounded double of
+ * each decimal text (Python's float(); nan and inf parse).  *nrows_out: the number of lines after the header; with
+ * CKM_ECAPACITY (more than row_cap) nothing is parsed.  An empty file, a line with another number of columns or a value
+ * that is not a number gives CKM_EFORMAT naming the line. */
+int  ckm_parse_kmer_profiles(const char *text, int64_t n, int32_t ncols, int32_t nthreads, int64_t *id_start_out,
+                             int32_t *id_len_out, double *values_out, int64_t row_cap, int64_t *nrows_out);
+/* A profile matrix (nrows x 136 float64, row-major) resident on the engine's device for the calls of one run. */
+typedef struct ckm_sigs ckm_sigs;
+int  ckm_sigs_create(ckm_engine *e, const double *values, int64_t nrows, ckm_sigs **out);
+void ckm_sigs_free(ckm_sigs *s);
+typedef struct {
+  int64_t nseq;                    /* sequences of the batch, the bins' back to back in dictionary order */
+  int32_t nbins, ntables;
+  const int64_t *bin_off;          /* nbins + 1: bin b holds sequences bin_off[b] .. bin_off[b+1] (at least one) */
+  const int64_t *len;              /* nseq: len(seq) >= 1 */
+  const int64_t *acgt;             /* nseq x 4: A, C, G, T-or-U of the upper-cased sequence (their sum >= 1) */
+  const int64_t *coding;           /* nseq: bases under at least one gene */
+  const int64_t *sig_row;          /* nseq: the sequence's row of the profile matrix */
+  const int32_t *bin_gc_table;     /* nbins: the bound table the bin's delta GC is held to ... */
+  const int32_t *bin_cd_table;     /* ... and its delta CD */
+  int32_t td_table, pad;           /* the bound table every TD is held to */
+  const int64_t *table_off;        /* ntables + 1: table t is entries table_off[t] .. table_off[t+1] (at least one) */
+  const double *table_key;         /* length keys in the distribution file's order */
+  const double *table_lo;          /* lower bound at the key (GC, CD tables) */
+  const double *table_hi;          /* upper bound at the key (GC, TD tables) */
+  const double *binsig_in;         /* optional, nbins x 136: bin signatures to measure TD against in place of the computed ones */
+} ckm_outlier_in;
+typedef struct {
+  double *bin_means;               /* nbins x 3: meanGC, meanCD, meanTD */
+  double *bin_sig;                 /* optional, nbins x 136: the bins' signatures (binTools.py:186-201) */
+  double *seq_values;              /* nseq x 9: GC, deltaGC, CD, deltaCD, TD, GC lower, GC upper, CD lower, TD upper bound */
+  uint8_t *seq_mask;               /* nseq: 1 = outlying in GC, 2 = in CD, 4 = in TD (binTools.py:279-286) */
+  float kernel_ms[3];              /* bin, sequence and mean kernels by CUDA events */
+} ckm_outlier_out;
+/* replaces gcDist, codingDensityDist, binTetraSig, tetraDiffDist and the bound look-ups of identifyOutliers
+ * (binTools.py:148-209, 264-286) for all bins of the batch.  A bin without sequences, an empty sequence, one without
+ * A/C/G/T or without a signature row is refused with CKM_EINVAL naming it (the reference divides by zero or raises there). */
+int  ckm_outlier_scores(ckm_engine *e, const ckm_sigs *sigs, const ckm_outlier_in *in, ckm_outlier_out *out);
+
 /* ---- read coverage (`checkm coverage`; checkm/coverage.py:57-287): BGZF blocks inflated and BAM records walked and
  * classified on the device, nine int64 counters per reference.  The kernels and the anchor argument are described in
  * csrc/bam.cu. ---- */
