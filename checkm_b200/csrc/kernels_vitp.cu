@@ -34,161 +34,242 @@ constexpr uint32_t VP_TFLOORW = 0xC000C000u;     // -16384 | -16384 : floor of t
 __device__ __forceinline__ int vp_lo(uint32_t w) { return (int)(int16_t)(w & 0xffffu); }
 __device__ __forceinline__ int vp_hi(uint32_t w) { return (int)w >> 16; }
 
-// Work distribution.  Every class kernel reads the one survivor list of the bias filter.  A warp takes 32 consecutive
-// candidates at a time (from the class's cursor p.vit_work[cls]: dynamic, so the long ORFs at the end of the list do not
-// leave a tail; without a cursor, in static strides), each lane looks up the class of one of them -- one coalesced pass
-// over the list per kernel instead of a dependent two-load round trip per candidate and warp -- and the warp then scores
-// the ones that are its own, one after the other.
-template <int W, bool TSMEM>
-__global__ void __launch_bounds__(128) vitp_kernel(FilterParams p, int cls) {
-  extern __shared__ __align__(16) uint8_t vsm[];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, wpb = blockDim.x >> 5;
-  uint4 *tws = reinterpret_cast<uint4 *>(vsm) + (size_t)warp * W * 64;
-  const uint32_t sel = (lane == 0) ? 0x1054u : 0x3210u;
+// the two ways out of the stage besides the score list: the pass list (P <= F2) and the int32 kernels' redo list
+__device__ __forceinline__ void vit_pass(const FilterParams &p, const Candidate &cd) {
+  const int pos = atomicAdd(p.out_count, 1);
+  if (pos < p.out_cap) p.out[pos] = cd;
+  if (p.dense_passed != nullptr) atomicOr_u8(p.dense_passed, (int64_t)p.model_slot[cd.model] * p.nseq + cd.seq, 4);
+}
+__device__ __forceinline__ void vit_redo(const FilterParams &p, const Candidate &cd) {
+  const int pos = atomicAdd(p.redo_count, 1);
+  if (pos < p.redo_cap) p.redo[pos] = cd;
+}
+// lane-block class (index into BLK_Q) of a model's vq; -1: no class
+__device__ __forceinline__ int vitp_class(int vq) { return vq == 0 ? -1 : (vq <= 8 ? vq / 2 - 1 : vq / 4 + 1); }
+
+// Grouping the survivor list by (class, model), in three passes over p.in.  Count: pairs that need no packed scoring leave
+// here -- P already <= F2 to the pass list, models without a class to the redo list -- and the others are counted per model.
+// Scan (one CTA): each model's first position in p.vit_idx and first chunk, classes in BLK_Q order, models in index order
+// within a class.  Scatter: each pair's index into p.in at its model's next free position; the pair that opens a chunk writes
+// the chunk.  The order within a model is whatever the atomics make it: every pair is scored on its own and the kernels append
+// their results through atomics, so no result depends on it.
+__global__ void vit_count_kernel(FilterParams p, int32_t *cnt) {
   const int n = min(*p.in_count, p.in_cap);
-  int32_t *cursor = (p.vit_work != nullptr) ? p.vit_work + cls : nullptr;
-  for (int64_t it = 0;; ++it) {
-    int64_t base64;
-    if (cursor != nullptr) {
-      int b = 0;
-      if (lane == 0) b = atomicAdd(cursor, 32);
-      base64 = __shfl_sync(0xffffffffu, b, 0);
-    } else {
-      base64 = ((it * gridDim.x + blockIdx.x) * wpb + warp) * 32;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const Candidate cd = p.in[i];
+    if (!(cd.P > p.F2)) vit_pass(p, cd);
+    else if (p.ms[cd.model].vq == 0) vit_redo(p, cd);
+    else atomicAdd(cnt + cd.model, 1);
+  }
+}
+
+__global__ void __launch_bounds__(1024) vit_scan_kernel(FilterParams p, int32_t nmodels, const int32_t *cnt, int32_t *off, int32_t *choff) {
+  __shared__ int ws[2][32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int run_pairs = 0, run_chunks = 0;
+  for (int c = 0; c < N_BLK_CLASSES; ++c) {
+    if (threadIdx.x == 0) p.vit_cls_chunks[c] = run_chunks;
+    for (int b = 0; b < nmodels; b += 1024) {
+      const int m = b + threadIdx.x;
+      const int v = (m < nmodels && vitp_class(p.ms[m].vq) == c) ? cnt[m] : 0, h = (v + VITP_CHUNK - 1) / VITP_CHUNK;
+      int sv = v, sh = h;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const int a = __shfl_up_sync(0xffffffffu, sv, o), d = __shfl_up_sync(0xffffffffu, sh, o);
+        if (lane >= o) { sv += a; sh += d; }
+      }
+      if (lane == 31) { ws[0][warp] = sv; ws[1][warp] = sh; }
+      __syncthreads();
+      if (warp == 0) {
+        int tv = ws[0][lane], th = ws[1][lane];
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+          const int a = __shfl_up_sync(0xffffffffu, tv, o), d = __shfl_up_sync(0xffffffffu, th, o);
+          if (lane >= o) { tv += a; th += d; }
+        }
+        ws[0][lane] = tv; ws[1][lane] = th;
+      }
+      __syncthreads();
+      if (v > 0) {
+        off[m] = run_pairs + (warp ? ws[0][warp - 1] : 0) + sv - v;
+        choff[m] = run_chunks + (warp ? ws[1][warp - 1] : 0) + sh - h;
+      }
+      run_pairs += ws[0][31]; run_chunks += ws[1][31];
+      __syncthreads();
     }
-    if (base64 >= n) break;
-    const int base = (int)base64;
-    bool mine = false;
-    if (base + lane < n) {
-      const int vq = p.ms[p.in[base + lane].model].vq;
-      mine = (vq == 2 * W) || (W == 1 && vq == 0);
+  }
+  if (threadIdx.x == 0) p.vit_cls_chunks[N_BLK_CLASSES] = run_chunks;
+}
+
+__global__ void vit_scatter_kernel(FilterParams p, const int32_t *cnt, int32_t *fill, const int32_t *off, const int32_t *choff) {
+  const int n = min(*p.in_count, p.in_cap);
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const int m = p.in[i].model;
+    if (!(p.in[i].P > p.F2) || p.ms[m].vq == 0) continue;
+    const int r = atomicAdd(fill + m, 1), pos = off[m] + r;
+    p.vit_idx[pos] = i;
+    if (r % VITP_CHUNK == 0) p.vit_chunks[choff[m] + r / VITP_CHUNK] = make_int2(pos, off[m] + min(r + VITP_CHUNK, cnt[m]));
+  }
+}
+
+int launch_vit_group(const FilterParams &p, int32_t nmodels, int32_t *ws, int grid, cudaStream_t st) {
+  int32_t *cnt = ws, *fill = ws + nmodels, *off = ws + 2 * (size_t)nmodels, *choff = ws + 3 * (size_t)nmodels;
+  cudaError_t e = cudaMemsetAsync(ws, 0, sizeof(int32_t) * 2 * (size_t)nmodels, st);
+  if (e != cudaSuccess) return cuda_fail(e, "cudaMemsetAsync(vit groups)");
+  vit_count_kernel<<<grid, 256, 0, st>>>(p, cnt);
+  vit_scan_kernel<<<1, 1024, 0, st>>>(p, nmodels, cnt, off, choff);
+  vit_scatter_kernel<<<grid, 256, 0, st>>>(p, cnt, fill, off, choff);
+  e = cudaGetLastError();
+  return e == cudaSuccess ? CKM_OK : cuda_fail(e, "vit grouping launch");
+}
+
+// Work distribution.  vit_group_pairs (below) first orders the survivor list by (class, model) into p.vit_idx and cuts each
+// model's run into chunks of at most VITP_CHUNK pairs (p.vit_chunks; class c owns chunks [vit_cls_chunks[c],
+// vit_cls_chunks[c+1])).  A CTA claims one chunk at a time from its class's cursor p.vit_work[cls], copies that model's
+// emission words (KPAD x W x 32, 3.75 KB per W) -- and for W >= 6 its transitions (1 KB per W) -- into shared memory once,
+// and its warps then take the chunk's pairs one by one from a shared cursor.  The row loop reads emissions with one
+// conflict-free LDS.32 per word; for W <= 4 the transitions stay in registers, loaded once per chunk.
+constexpr int VITP_THREADS = 128;
+
+__host__ __device__ constexpr int vitp_smem_bytes(int W, bool tsmem) { return KPAD * W * 32 * 4 + (tsmem ? W * 64 * 16 : 0); }
+// CTAs per SM the register budget must allow: 4 warps per scheduler for W <= 4, 3 for W <= 10, 2 beyond
+__host__ __device__ constexpr int vitp_min_blocks(int W) { return W <= 4 ? 4 : (W <= 10 ? 3 : 2); }
+
+template <int W, bool TSMEM>
+__global__ void __launch_bounds__(VITP_THREADS, vitp_min_blocks(W)) vitp_kernel(FilterParams p, int cls) {
+  extern __shared__ __align__(16) uint4 vsm[];
+  __shared__ int s_chunk, s_next;
+  __shared__ ModelScalars s_ms;                                    // the chunk's model: read where used, not held in registers
+  uint32_t *esm = reinterpret_cast<uint32_t *>(vsm);              // [KPAD][W][32] emission words
+  uint4 *tws = vsm + KPAD * W * 8;                                 // [half][w][lane] transitions (TSMEM): conflict-free LDS.128
+  const int lane = threadIdx.x & 31;
+  const uint32_t sel = (lane == 0) ? 0x1054u : 0x3210u;
+  const int c0 = p.vit_cls_chunks[cls], nch = p.vit_cls_chunks[cls + 1] - c0;
+  for (;;) {
+    __syncthreads();                                               // every warp is done with the previous chunk's tables
+    if (threadIdx.x == 0) {
+      const int k = atomicAdd(p.vit_work + cls, 1);
+      s_chunk = k;
+      if (k < nch) {
+        s_next = p.vit_chunks[c0 + k].x;
+        s_ms = p.ms[p.in[p.vit_idx[s_next]].model];
+      }
     }
-    unsigned todo = __ballot_sync(0xffffffffu, mine);
-  while (todo != 0u) {
-    const int c = base + __ffs(todo) - 1;
-    todo &= todo - 1u;
-    Candidate cd = p.in[c];
-    const int m = cd.model;
-    const ModelScalars ms = p.ms[m];
-    const bool unclassed = (ms.vq == 0 && W == 1);      // the first class also forwards models without a class
-    if (ms.vq != 2 * W && !unclassed) continue;
-    const int s = cd.seq, L = p.len[s];
-    bool pass = true, redo = false;
-    if (cd.P > p.F2) {
+    __syncthreads();
+    const int k = s_chunk;
+    if (k >= nch) break;
+    const int2 ch = p.vit_chunks[c0 + k];
+    const ModelScalars &ms = s_ms;
+    {
+      const uint4 *esrc = reinterpret_cast<const uint4 *>(p.rwp + ms.blk_off * 32 * (KPAD / 2));
+      for (int z = threadIdx.x; z < KPAD * W * 8; z += VITP_THREADS) vsm[z] = __ldg(esrc + z);
+      if (TSMEM) {
+        const uint4 *tsrc = p.twp + ms.blk_off * 32;
+        for (int z = threadIdx.x; z < W * 64; z += VITP_THREADS) tws[(z & 1) * (W * 32) + (z >> 1)] = __ldg(tsrc + z);
+      }
+    }
+    uint4 tr0[TSMEM ? 1 : W], tr1[TSMEM ? 1 : W];
+    if (!TSMEM) {
+      const uint4 *tsrc = p.twp + ms.blk_off * 32;
+#pragma unroll
+      for (int w = 0; w < W; ++w) { tr0[TSMEM ? 0 : w] = __ldg(tsrc + (w * 32 + lane) * 2); tr1[TSMEM ? 0 : w] = __ldg(tsrc + (w * 32 + lane) * 2 + 1); }
+    }
+#define TR0(w) (TSMEM ? tws[(w) * 32 + lane] : tr0[TSMEM ? 0 : (w)])
+#define TR1(w) (TSMEM ? tws[W * 32 + (w) * 32 + lane] : tr1[TSMEM ? 0 : (w)])
+    __syncthreads();
+    const uint32_t *erow = esm + lane;
+    const int ddbound = ms.ddbound_w, cap = 32767 - (int)ms.vit_emax;
+    const int e_move = ms.xw_e_move, e_loop = ms.xw_e_loop;
+    for (;;) {
+      int j = 0;
+      if (lane == 0) j = atomicAdd(&s_next, 1);
+      j = __shfl_sync(0xffffffffu, j, 0);
+      if (j >= ch.y) break;
+      const Candidate *cin = p.in + p.vit_idx[j];      // read again after the row loop rather than held through it
+      const int s = cin->seq, L = p.len[s];
+      bool redo = false;
       const int tmove = p.tmove_w[s];
       const int cost = -tmove - (int)ms.vit_tbm + 64;
       const bool c1 = (cost - (int)ms.xw_e_loop <= 22528) && (cost <= 22240);
       const bool c1p = (cost - (int)ms.xw_e_loop <= 16384);
-      redo = unclassed || !c1;
+      redo = !c1;
       float vsc = 0.0f;
       if (!redo) {
-        uint4 tr0[TSMEM ? 1 : W], tr1[TSMEM ? 1 : W];
-        const uint4 *tsrc = p.twp + ms.blk_off * 32;
-        if (TSMEM) {
-          __syncwarp();
-          for (int z = lane; z < W * 64; z += 32) tws[(z & 1) * (W * 32) + (z >> 1)] = __ldg(tsrc + z);     // [half][w][lane]: conflict-free LDS.128
-          __syncwarp();
-        } else {
-#pragma unroll
-          for (int w = 0; w < W; ++w) { tr0[TSMEM ? 0 : w] = __ldg(tsrc + (w * 32 + lane) * 2); tr1[TSMEM ? 0 : w] = __ldg(tsrc + (w * 32 + lane) * 2 + 1); }
-        }
-#define TR0(w) (TSMEM ? tws[(w) * 32 + lane] : tr0[TSMEM ? 0 : (w)])
-#define TR1(w) (TSMEM ? tws[W * 32 + (w) * 32 + lane] : tr1[TSMEM ? 0 : (w)])
-        const uint32_t *rwp = p.rwp + ms.blk_off * 32 * (KPAD / 2) + lane;
         uint32_t Mx[W], Ix[W], Dx[W];
 #pragma unroll
         for (int w = 0; w < W; ++w) { Mx[w] = VP_FLOORW; Ix[w] = VP_FLOORW; Dx[w] = VP_FLOORW; }
-        const int ddbound = ms.ddbound_w, cap = 32767 - (int)ms.vit_emax;
-        const int e_move = ms.xw_e_move, e_loop = ms.xw_e_loop;
         int xN = ms.base_w, xB = xN + tmove, xJ = -32768, xC = -32768;
-        const uint4 *rp = reinterpret_cast<const uint4 *>(p.res + p.off[s]);
-        const int nblk = (L + 15) >> 4;
-        uint4 r16 = (nblk > 0) ? __ldg(rp) : make_uint4(0, 0, 0, 0);
-        uint32_t ecur[W];
-        {
-          const uint32_t x0 = r16.x & 0xffu;
-#pragma unroll
-          for (int w = 0; w < W; ++w) ecur[w] = __ldg(rwp + (x0 * W + w) * 32);
-        }
+        // residues 4 at a time, the next word requested one group of rows ahead
+        const uint32_t *rp = reinterpret_cast<const uint32_t *>(p.res + p.off[s]);
+        const int nw = (L + 3) >> 2;
+        uint32_t wcur = (nw > 0) ? __ldg(rp) : 0u;
         bool stop = false;
-        for (int b = 0; b < nblk && !stop; ++b) {
-          const uint4 rnext = (b + 1 < nblk) ? __ldg(rp + b + 1) : make_uint4(0, 0, 0, 0);
-          for (int j = 0; j < 4 && !stop; ++j) {
-            const uint32_t wcur = (j == 0) ? r16.x : (j == 1) ? r16.y : (j == 2) ? r16.z : r16.w;
-            const uint32_t wnxt = (j == 0) ? r16.y : (j == 1) ? r16.z : (j == 2) ? r16.w : rnext.x;
+        for (int q = 0; q < nw && !stop; ++q) {
+          const uint32_t wnext = (q + 1 < nw) ? __ldg(rp + q + 1) : 0u;
 #pragma unroll
-            for (int rr = 0; rr < 4; ++rr) {
-              if (b * 16 + j * 4 + rr >= L) { stop = true; break; }
-              // emission words of the NEXT row are requested now and consumed one iteration later
-              uint32_t enext[W];
-              {
-                const uint32_t xn = (rr < 3) ? ((wcur >> (8 * (rr + 1))) & 0xffu) : (wnxt & 0xffu);
+          for (int rr = 0; rr < 4; ++rr) {
+            if (q * 4 + rr >= L) { stop = true; break; }
+            const uint32_t *ew = erow + ((wcur >> (8 * rr)) & 0xffu) * (W * 32);
+            // row i-1 values of the position just below my block, both halves
+            const uint32_t shM = __shfl_sync(0xffffffffu, Mx[W - 1], (lane + 31) & 31);
+            const uint32_t shI = __shfl_sync(0xffffffffu, Ix[W - 1], (lane + 31) & 31);
+            const uint32_t shD = __shfl_sync(0xffffffffu, Dx[W - 1], (lane + 31) & 31);
+            const uint32_t pm0 = __byte_perm(shM, VP_FLOORW, sel), pi0 = __byte_perm(shI, VP_FLOORW, sel), pd0 = __byte_perm(shD, VP_FLOORW, sel);
+            const uint32_t xBw = __byte_perm((uint32_t)xB, 0u, 0x1010u);
+            uint32_t md[W];
+            uint32_t xEw = VP_FLOORW, dmw = VP_FLOORW;
 #pragma unroll
-                for (int w = 0; w < W; ++w) enext[w] = __ldg(rwp + (xn * W + w) * 32);
+            for (int w = W - 1; w >= 0; --w) {
+              const uint32_t pm = (w > 0) ? Mx[w - 1] : pm0, pi = (w > 0) ? Ix[w - 1] : pi0, pd = (w > 0) ? Dx[w - 1] : pd0;
+              const uint4 t0 = TR0(w), t1 = TR1(w);
+              uint32_t sv = __viaddmax_s16x2(xBw, t0.x, VP_FLOORW);
+              sv = __viaddmax_s16x2(pm, t0.y, sv);
+              sv = __viaddmax_s16x2(pi, t0.z, sv);
+              sv = __viaddmax_s16x2(pd, t0.w, sv);
+              sv = __viaddmax_s16x2(sv, ew[w * 32], VP_FLOORW);
+              const uint32_t nI = __viaddmax_s16x2(Ix[w], t1.z, __viaddmax_s16x2(Mx[w], t1.y, VP_FLOORW));
+              md[w] = __viaddmax_s16x2(sv, t1.x, VP_FLOORW);
+              Mx[w] = sv; Ix[w] = nI;
+            }
+#pragma unroll
+            for (int w = 0; w + 1 < W; w += 2) { xEw = __vimax3_s16x2(xEw, Mx[w], Mx[w + 1]); dmw = __vimax3_s16x2(dmw, md[w], md[w + 1]); }
+            if (W & 1) { xEw = __vimax3_s16x2(xEw, Mx[W - 1], Mx[W - 1]); dmw = __vimax3_s16x2(dmw, md[W - 1], md[W - 1]); }
+            const int xE = __reduce_max_sync(0xffffffffu, max(vp_lo(xEw), vp_hi(xEw)));
+            if (xE >= cap) { redo = true; stop = true; break; }
+            xC = max(xC, xE + e_move);
+            xJ = max(xJ, xE + e_loop);
+            xB = max(xJ + tmove, xN + tmove);
+            const int Dmax = __reduce_max_sync(0xffffffffu, max(vp_lo(dmw), vp_hi(dmw)));
+            if (Dmax + ddbound > xB) {
+              if (!c1p) { redo = true; stop = true; break; }
+              // full D->D.  Per lane and half: composite f(d) = max(Bb, d + Tb) of my W cells; inclusive max-plus scan over
+              // the lanes (the two halves are two independent chains here); then the high chain takes the low chain's exit.
+              uint32_t Bb = VP_FLOORW, Tb = 0u;
+#pragma unroll
+              for (int w = 0; w < W; ++w) { const uint32_t tdd = TR1(w).w; Bb = __viaddmax_s16x2(Bb, tdd, md[w]); Tb = __viaddmax_s16x2(Tb, __vimax3_s16x2(tdd, VP_TFLOORW, VP_TFLOORW), VP_TFLOORW); }
+              uint32_t Bs = Bb, Ts = Tb;
+#pragma unroll
+              for (int o = 1; o < 32; o <<= 1) {
+                const uint32_t Bl = __shfl_up_sync(0xffffffffu, Bs, o), Tl = __shfl_up_sync(0xffffffffu, Ts, o);
+                if (lane >= o) { Bs = __viaddmax_s16x2(Bl, Ts, Bs); Ts = __viaddmax_s16x2(Ts, Tl, VP_TFLOORW); }
               }
-              // row i-1 values of the position just below my block, both halves
-              const uint32_t shM = __shfl_sync(0xffffffffu, Mx[W - 1], (lane + 31) & 31);
-              const uint32_t shI = __shfl_sync(0xffffffffu, Ix[W - 1], (lane + 31) & 31);
-              const uint32_t shD = __shfl_sync(0xffffffffu, Dx[W - 1], (lane + 31) & 31);
-              const uint32_t pm0 = __byte_perm(shM, VP_FLOORW, sel), pi0 = __byte_perm(shI, VP_FLOORW, sel), pd0 = __byte_perm(shD, VP_FLOORW, sel);
-              const uint32_t xBw = __byte_perm((uint32_t)xB, 0u, 0x1010u);
-              uint32_t md[W];
-              uint32_t xEw = VP_FLOORW, dmw = VP_FLOORW;
+              uint32_t din = __shfl_up_sync(0xffffffffu, Bs, 1), Tex = __shfl_up_sync(0xffffffffu, Ts, 1);
+              if (lane == 0) { din = VP_FLOORW; Tex = 0u; }
+              const uint32_t lowexit = __shfl_sync(0xffffffffu, Bs, 31);                 // low half: D(i, 32W+1)
+              const uint32_t dmid = __byte_perm(lowexit, VP_FLOORW, 0x1054u);            // (low: FLOOR, high: that exit)
+              din = __viaddmax_s16x2(dmid, Tex, din);
+              uint32_t d = din;
 #pragma unroll
-              for (int w = W - 1; w >= 0; --w) {
-                const uint32_t pm = (w > 0) ? Mx[w - 1] : pm0, pi = (w > 0) ? Ix[w - 1] : pi0, pd = (w > 0) ? Dx[w - 1] : pd0;
-                const uint4 t0 = TR0(w), t1 = TR1(w);
-                uint32_t sv = __viaddmax_s16x2(xBw, t0.x, VP_FLOORW);
-                sv = __viaddmax_s16x2(pm, t0.y, sv);
-                sv = __viaddmax_s16x2(pi, t0.z, sv);
-                sv = __viaddmax_s16x2(pd, t0.w, sv);
-                sv = __viaddmax_s16x2(sv, ecur[w], VP_FLOORW);
-                const uint32_t nI = __viaddmax_s16x2(Ix[w], t1.z, __viaddmax_s16x2(Mx[w], t1.y, VP_FLOORW));
-                md[w] = __viaddmax_s16x2(sv, t1.x, VP_FLOORW);
-                Mx[w] = sv; Ix[w] = nI;
-              }
+              for (int w = 0; w < W; ++w) { Dx[w] = d; d = __viaddmax_s16x2(d, TR1(w).w, md[w]); }
+            } else {
+              // lazy F: no D->D path can beat entering from B; D(i,k) = M(i,k-1) + tMD(k-1)
+              const uint32_t shd = __shfl_sync(0xffffffffu, md[W - 1], (lane + 31) & 31);
 #pragma unroll
-              for (int w = 0; w + 1 < W; w += 2) { xEw = __vimax3_s16x2(xEw, Mx[w], Mx[w + 1]); dmw = __vimax3_s16x2(dmw, md[w], md[w + 1]); }
-              if (W & 1) { xEw = __vimax3_s16x2(xEw, Mx[W - 1], Mx[W - 1]); dmw = __vimax3_s16x2(dmw, md[W - 1], md[W - 1]); }
-              const int xE = __reduce_max_sync(0xffffffffu, max(vp_lo(xEw), vp_hi(xEw)));
-              if (xE >= cap) { redo = true; stop = true; break; }
-              xC = max(xC, xE + e_move);
-              xJ = max(xJ, xE + e_loop);
-              xB = max(xJ + tmove, xN + tmove);
-              const int Dmax = __reduce_max_sync(0xffffffffu, max(vp_lo(dmw), vp_hi(dmw)));
-              if (Dmax + ddbound > xB) {
-                if (!c1p) { redo = true; stop = true; break; }
-                // full D->D.  Per lane and half: composite f(d) = max(Bb, d + Tb) of my W cells; inclusive max-plus scan over
-                // the lanes (the two halves are two independent chains here); then the high chain takes the low chain's exit.
-                uint32_t Bb = VP_FLOORW, Tb = 0u;
-#pragma unroll
-                for (int w = 0; w < W; ++w) { const uint32_t tdd = TR1(w).w; Bb = __viaddmax_s16x2(Bb, tdd, md[w]); Tb = __viaddmax_s16x2(Tb, __vimax3_s16x2(tdd, VP_TFLOORW, VP_TFLOORW), VP_TFLOORW); }
-                uint32_t Bs = Bb, Ts = Tb;
-#pragma unroll
-                for (int o = 1; o < 32; o <<= 1) {
-                  const uint32_t Bl = __shfl_up_sync(0xffffffffu, Bs, o), Tl = __shfl_up_sync(0xffffffffu, Ts, o);
-                  if (lane >= o) { Bs = __viaddmax_s16x2(Bl, Ts, Bs); Ts = __viaddmax_s16x2(Ts, Tl, VP_TFLOORW); }
-                }
-                uint32_t din = __shfl_up_sync(0xffffffffu, Bs, 1), Tex = __shfl_up_sync(0xffffffffu, Ts, 1);
-                if (lane == 0) { din = VP_FLOORW; Tex = 0u; }
-                const uint32_t lowexit = __shfl_sync(0xffffffffu, Bs, 31);                 // low half: D(i, 32W+1)
-                const uint32_t dmid = __byte_perm(lowexit, VP_FLOORW, 0x1054u);            // (low: FLOOR, high: that exit)
-                din = __viaddmax_s16x2(dmid, Tex, din);
-                uint32_t d = din;
-#pragma unroll
-                for (int w = 0; w < W; ++w) { Dx[w] = d; d = __viaddmax_s16x2(d, TR1(w).w, md[w]); }
-              } else {
-                // lazy F: no D->D path can beat entering from B; D(i,k) = M(i,k-1) + tMD(k-1)
-                const uint32_t shd = __shfl_sync(0xffffffffu, md[W - 1], (lane + 31) & 31);
-#pragma unroll
-                for (int w = W - 1; w >= 1; --w) Dx[w] = md[w - 1];
-                Dx[0] = __byte_perm(shd, VP_FLOORW, sel);
-              }
-#pragma unroll
-              for (int w = 0; w < W; ++w) ecur[w] = enext[w];
+              for (int w = W - 1; w >= 1; --w) Dx[w] = md[w - 1];
+              Dx[0] = __byte_perm(shd, VP_FLOORW, sel);
             }
           }
-          r16 = rnext;
+          wcur = wnext;
         }
         if (!redo && xC <= VP_FLOOR + e_move) redo = true;      // a floored row may have set xC (or nothing scored at all)
         if (!redo) {
@@ -196,40 +277,34 @@ __global__ void __launch_bounds__(128) vitp_kernel(FilterParams p, int cls) {
           vsc = __fdiv_rn(vsc, ms.scale_w);
           vsc = __fsub_rn(vsc, 3.0f);
         }
-#undef TR0
-#undef TR1
       }
+      Candidate cd = *cin;
       if (redo) {
-        if (lane == 0) {
-          const int pos = atomicAdd(p.redo_count, 1);
-          if (pos < p.redo_cap) p.redo[pos] = cd;
-        }
+        if (lane == 0) vit_redo(p, cd);
         continue;
       }
       cd.vitsc = vsc;
       const float seq_score = __fdiv_rn(__fsub_rn(vsc, cd.filtersc), 0.69314718055994529f);
       const double P = gumbel_surv((double)seq_score, (double)ms.evparam[2], (double)ms.evparam[3]);
       cd.P = P;
-      pass = (P <= p.F2);
-      if (lane == 0 && p.dense_vit != nullptr) p.dense_vit[(int64_t)p.model_slot[m] * p.nseq + s] = vsc;
-    }
-    if (lane == 0 && pass) {
-      const int pos = atomicAdd(p.out_count, 1);
-      if (pos < p.out_cap) p.out[pos] = cd;
-      if (p.dense_passed != nullptr) atomicOr_u8(p.dense_passed, (int64_t)p.model_slot[m] * p.nseq + s, 4);
-    }
-  }   // candidates of this group of 32
-  }   // groups
+      if (lane == 0) {
+        if (p.dense_vit != nullptr) p.dense_vit[(int64_t)p.model_slot[cd.model] * p.nseq + s] = vsc;
+        if (P <= p.F2) vit_pass(p, cd);
+      }
+    }   // pairs of this chunk
+#undef TR0
+#undef TR1
+  }   // chunks
 }
 
 template <int W, bool TSMEM>
 static int launch_vitp_w(const FilterParams &p, int cls, int grid, cudaStream_t st) {
-  const int sm = TSMEM ? 4 * W * 64 * (int)sizeof(uint4) : 0;
+  constexpr int sm = vitp_smem_bytes(W, TSMEM);
   if (sm > 48 * 1024) {
     cudaError_t e = cudaFuncSetAttribute(vitp_kernel<W, TSMEM>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm);
     if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(vitp)");
   }
-  vitp_kernel<W, TSMEM><<<grid, 128, sm, st>>>(p, cls);
+  vitp_kernel<W, TSMEM><<<grid, VITP_THREADS, sm, st>>>(p, cls);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? CKM_OK : cuda_fail(e, "vitp_kernel launch");
 }

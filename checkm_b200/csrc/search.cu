@@ -315,14 +315,26 @@ static int run_stage1(ckm_engine *e, const SearchKnobs &k, const ckm_models *m, 
   return CKM_OK;
 }
 
-// ViterbiFilter from p.in to p.out.  packed: the int16x2 kernels, one per class, score first; what they cannot score exactly
-// (strong hits near the int16 ceiling, models without a class, pairs outside the safety conditions of kernels_vitp.cu) lands
-// in the redo list, which the int32 kernels then take as their input.
-static int run_viterbi(ckm_engine *e, FilterParams &p, bool packed) {
+// ViterbiFilter from p.in to p.out.  packed: the int16x2 kernels, one per class, score first, from an index list grouped
+// by (class, model) in `grp`; what they cannot score exactly (strong hits near the int16 ceiling, models without a class,
+// pairs outside the safety conditions of kernels_vitp.cu) lands in the redo list, which the int32 kernels then take as their
+// input.  No stage depends on the order of its input list: every kernel appends through atomics, and sorted_pairs orders the
+// Forward survivors on the host.
+static int run_viterbi(ckm_engine *e, const ckm_models *m, FilterParams &p, bool packed, DevBuf &grp) {
   int rc;
   if (packed) {
+    const int nm = (int)m->models.size();
+    const size_t nchunks = (size_t)p.in_cap / VITP_CHUNK + nm + 1;           // every model's last chunk may be partial
+    const size_t words = 4 * (size_t)nm + 16 + ((size_t)p.in_cap + 1) / 2 * 2;
+    if ((rc = grp.alloc(sizeof(int32_t) * words + sizeof(int2) * nchunks))) return rc;
+    int32_t *ws = grp.as<int32_t>();
+    p.vit_cls_chunks = ws + 4 * (size_t)nm;
+    p.vit_idx = p.vit_cls_chunks + 16;
+    p.vit_chunks = reinterpret_cast<int2 *>(ws + words);
     p.vit_work = e->d_counters + CTR_VWORK;      // zeroed with the other counters at the start of the call
+    if ((rc = launch_vit_group(p, nm, ws, e->prop.multiProcessorCount * 8, e->stream))) return rc;
     if ((rc = per_class<FilterParams>(e, p, launch_vitp, 8, nullptr, 0))) return rc;
+    e->stats.kernel_launches += 3;
     p.in = p.redo; p.in_count = p.redo_count; p.in_cap = p.redo_cap;
   }
   // lane-blocked register kernels, one per class; models beyond the classes (all models without use_blk): shared-memory rows
@@ -330,7 +342,7 @@ static int run_viterbi(ckm_engine *e, FilterParams &p, bool packed) {
 }
 // Stages 2-4 on the MSV survivors: bias filter -> ViterbiFilter -> ForwardParser.  Lists ping-pong between two buffers.
 struct Stage2 {
-  DevBuf a, b, redo;      // the survivors of the Forward filter end in a
+  DevBuf a, b, redo, vgrp;      // the survivors of the Forward filter end in a; vgrp: the packed Viterbi work list
   int32_t cap = 0;
 };
 static int run_stage2(ckm_engine *e, const SearchKnobs &k, const ckm_models *m, const ckm_seqdb *db, ActiveMasks &am, Stage1 &s1, Stage2 &s2,
@@ -354,7 +366,7 @@ static int run_stage2(ckm_engine *e, const SearchKnobs &k, const ckm_models *m, 
   // viterbi: a -> b
   p.in = s2.a.as<Candidate>(); p.in_count = e->d_counters + CTR_BIAS; p.in_cap = s2.cap;
   p.out = s2.b.as<Candidate>(); p.out_count = e->d_counters + CTR_VIT; p.out_cap = s2.cap;
-  if ((rc = run_viterbi(e, p, k.vitp))) return rc;
+  if ((rc = run_viterbi(e, m, p, k.vitp, s2.vgrp))) return rc;
   CKM_CUDA(cudaEventRecord(e->ev[EV_FWD], st));
   // forward: b -> a
   p.in = s2.b.as<Candidate>(); p.in_count = e->d_counters + CTR_VIT; p.in_cap = s2.cap;
@@ -913,7 +925,7 @@ int ckm_viterbi_scores(ckm_engine *e, const ckm_models *m, const int32_t *model_
   std::vector<int32_t> slot_model((size_t)std::max(nmodels, 1));
   for (int i = 0; i < nmodels; ++i) slot_model[i] = model_idx ? model_idx[i] : i;
   const size_t nf = (size_t)std::max<int64_t>(n, 1);
-  DevBuf dsm, din, dout, dredo, dvit;
+  DevBuf dsm, din, dout, dredo, dvit, dgrp;
   if ((rc = dsm.alloc(sizeof(int32_t) * slot_model.size())) || (rc = din.alloc(sizeof(Candidate) * nf)) || (rc = dout.alloc(sizeof(Candidate) * nf)) ||
       (rc = dredo.alloc(sizeof(Candidate) * nf)) || (rc = dvit.alloc(sizeof(float) * nf))) return rc;
   CKM_CUDA(cudaMemcpyAsync(dsm.p, slot_model.data(), sizeof(int32_t) * slot_model.size(), cudaMemcpyHostToDevice, st));
@@ -928,7 +940,7 @@ int ckm_viterbi_scores(ckm_engine *e, const ckm_models *m, const int32_t *model_
     p.redo = dredo.as<Candidate>(); p.redo_count = e->d_counters + CTR_VREDO; p.redo_cap = (int32_t)nf;
     p.in = din.as<Candidate>(); p.in_count = e->d_counters + CTR_BIAS; p.in_cap = (int32_t)nf;
     p.out = dout.as<Candidate>(); p.out_count = e->d_counters + CTR_VIT; p.out_cap = (int32_t)nf;
-    if ((rc = run_viterbi(e, p, mode == 0))) return rc;
+    if ((rc = run_viterbi(e, m, p, mode == 0, dgrp))) return rc;
   }
   int32_t ctr[CTR_N];
   CKM_CUDA(cudaMemcpyAsync(ctr, e->d_counters, sizeof(ctr), cudaMemcpyDeviceToHost, st));

@@ -74,7 +74,9 @@ struct FilterParams {
   const uint4 *twb; const uint32_t *rwb; const float4 *tfb; const float *rfb;   // lane-blocked tables
   const uint4 *twp; const uint32_t *rwp;                                         // packed Viterbi tables
   Candidate *redo; int32_t *redo_count; int32_t redo_cap;                       // pairs the packed Viterbi kernel hands to the int32 kernels
-  int32_t *vit_work;                 // N_BLK_CLASSES zeroed cursors into `in`, one per packed-Viterbi class kernel (null: static strides)
+  // packed Viterbi work list (launch_vit_group): indices into `in` grouped by (class, model), chunks {begin, end} of at most
+  // VITP_CHUNK of them, class c owning chunks [vit_cls_chunks[c], vit_cls_chunks[c+1]); vit_work: N_BLK_CLASSES zeroed chunk cursors
+  int32_t *vit_idx; int2 *vit_chunks; int32_t *vit_cls_chunks; int32_t *vit_work;
   const Candidate *in; const int32_t *in_count; int32_t in_cap;
   Candidate *out; int32_t *out_count; int32_t out_cap;
   int32_t row_elems;                 // shared-memory elements of one DP row
@@ -91,6 +93,9 @@ constexpr int N_BLK_CLASSES = 10;
 constexpr int BLK_Q[N_BLK_CLASSES] = {2, 4, 6, 8, 12, 16, 20, 24, 28, 32};
 int launch_vit2(const FilterParams &p, int cls, int grid, cudaStream_t st);
 int launch_vitp(const FilterParams &p, int cls, int grid, cudaStream_t st);   // packed int16x2 kernels (kernels_vitp.cu)
+constexpr int VITP_CHUNK = 64;      // pairs of one model a packed-Viterbi CTA takes at a time
+// the packed kernels' work list from p.in; ws: 4 * nmodels int32 of scratch.  Pairs that need no packed scoring go to p.out / p.redo here.
+int launch_vit_group(const FilterParams &p, int32_t nmodels, int32_t *ws, int grid, cudaStream_t st);
 int launch_all_pairs(Candidate *out, int32_t *count, const int32_t *slot_model, int32_t nslots, int32_t nseq, cudaStream_t st);
 int launch_fwd(const FilterParams &p, int grid, cudaStream_t st);
 
