@@ -87,7 +87,7 @@ SYMBOLS = ["ckm_init", "ckm_destroy", "ckm_last_error", "ckm_version", "ckm_devi
            "ckm_filter_scores", "ckm_viterbi_scores", "ckm_write_domtblout", "ckm_reduce", "ckm_genome_check", "ckm_free", "ckm_allgather_qa", "ckm_nccl_unique_id",
            "ckm_nccl_comm_init", "ckm_nccl_comm_destroy", "ckm_fasta_scan_nt", "ckm_scaffold_stats",
            "ckm_kmer_counts", "ckm_kmer_columns", "ckm_format_kmer_profiles", "ckm_merge_pairs", "ckm_format_merger_rows",
-           "ckm_bgzf_blocks", "ckm_bgzf_inflate", "ckm_bam_coverage",
+           "ckm_bgzf_blocks", "ckm_bgzf_inflate", "ckm_bam_coverage", "ckm_bam_windows",
            "ckm_parse_kmer_profiles", "ckm_sigs_create", "ckm_sigs_free", "ckm_outlier_scores"]
 
 _lib = None
@@ -133,6 +133,8 @@ def lib():
     L.ckm_bgzf_blocks.argtypes = [vp, i64, i64, vp, i64, C.POINTER(i64), C.POINTER(i64)]
     L.ckm_bgzf_inflate.argtypes = [vp, vp, i64, i64, vp, i64, vp, i64, C.POINTER(i64), C.POINTER(C.c_float)]
     L.ckm_bam_coverage.argtypes = [vp, vp, i64, i64, vp, i64, vp, vp, i64, i32, C.POINTER(BamFilter), vp, vp, C.POINTER(i64)]
+    L.ckm_bam_windows.argtypes = [vp, vp, i64, i64, vp, i64, vp, vp, i64, i32, C.POINTER(BamFilter), vp, i64, vp, vp, vp, vp,
+                                  C.POINTER(i64)]
     L.ckm_seqdb_create.argtypes = [vp, vp, vp, i32, vp, i32, C.POINTER(vp)]
     L.ckm_seqdb_free.argtypes = [vp]
     L.ckm_seqdb_free.restype = None

@@ -40,6 +40,29 @@ def batch_bytes():
     return int(float(os.environ.get('CKM_BAM_BATCH_MB', str(DEFAULT_BATCH_MB))) * (1 << 20))
 
 
+def print_summary(logger, cnt, numRefSeqs):
+    """The summary the reference's writer prints per BAM (coverage.py:258-287, coverageWindows.py:243-255: the same text)
+    from the n_ref x 9 counters, when the logger shows INFO."""
+    if logger.getEffectiveLevel() > logging.INFO:
+        return
+    if numRefSeqs:
+        sys.stderr.write('    Finished processing %d of %d (%.2f%%) reference sequences.\r' %
+                         (numRefSeqs, numRefSeqs, 100.0))
+    sys.stderr.write('\n')
+    sys.stderr.flush()
+    t = cnt.sum(axis=0).tolist() if len(cnt) else [0] * 9
+    total = t[0]
+    print('')
+    print('    # total reads: %d' % total)
+    if total == 0:                    # the reference divides by the total here and its writer process stops
+        return
+    for label, v in (('properly mapped reads', t[7]), ('duplicate reads', t[1]), ('secondary reads', t[2]),
+                     ('reads failing QC', t[3]), ('reads failing alignment length', t[4]),
+                     ('reads failing edit distance', t[5]), ('reads not properly paired', t[6])):
+        print('      # %s: %d (%.1f%%)' % (label, v, float(v) * 100 / total))
+    print('')
+
+
 class Coverage():
     """Calculate coverage of all sequences."""
 
@@ -139,24 +162,7 @@ class Coverage():
 
     def _summary(self, cnt, numRefSeqs):
         """The per-BAM summary of coverage.py:258-287 (stdout), when the logger shows INFO."""
-        if self.logger.getEffectiveLevel() > logging.INFO:
-            return
-        if numRefSeqs:
-            sys.stderr.write('    Finished processing %d of %d (%.2f%%) reference sequences.\r' %
-                             (numRefSeqs, numRefSeqs, 100.0))
-        sys.stderr.write('\n')
-        sys.stderr.flush()
-        t = cnt.sum(axis=0).tolist() if len(cnt) else [0] * 9
-        total = t[0]
-        print('')
-        print('    # total reads: %d' % total)
-        if total == 0:                    # the reference divides by the total here and its writer process stops
-            return
-        for label, v in (('properly mapped reads', t[7]), ('duplicate reads', t[1]), ('secondary reads', t[2]),
-                         ('reads failing QC', t[3]), ('reads failing alignment length', t[4]),
-                         ('reads failing edit distance', t[5]), ('reads not properly paired', t[6])):
-            print('      # %s: %d (%.1f%%)' % (label, v, float(v) * 100 / total))
-        print('')
+        print_summary(self.logger, cnt, numRefSeqs)
 
     def parseCoverage(self, coverageFile):
         """{binId: {seqId: {bamId: coverage}}} of a coverage file."""

@@ -24,6 +24,14 @@
 //                        record start taken from the BAI's linear index) and every record start is verified; an index
 //                        that belongs to another file, or a truncated file, gives CKM_EFORMAT, never a wrong table.
 //                        The walk stops at the first record with refID -1 (the unplaced tail).
+//   bam_window_kernel    `checkm gc_bias_plot`'s read depth (coverageWindows.py:55-79): the same segments, the same record
+//                        decode, bounds checks and NM look-up, but coverageWindows' classification and the fetch rule of
+//                        `fetch(ref, 0, len)`.  Each mapped read adds its clipped span [pos, min(pos + alen, len)) to its
+//                        reference's covered bases and each window's overlap with it to an int64 window array.  The
+//                        thread keeps one (window, partial sum) in registers and flushes it with a 64-bit atomic when the
+//                        window changes; the reads are coordinate-sorted, so most reads land in the cached window.  Walkers
+//                        of neighbouring segments may share a window (segments end on 16 kbp index windows, not on W), and
+//                        the atomics make that correct.
 #include <algorithm>
 #include <cstdint>
 #include <cstdio>
@@ -327,15 +335,20 @@ __global__ void __launch_bounds__(IW * 32) bgzf_inflate_kernel(InflateParams p) 
 }
 
 // ---- the record walk ----
-enum { SC_OK = 0, SC_RECORD, SC_REFID, SC_UNPLACED, SC_NO_NM, SC_ANCHOR, SC_AUX, SC_NCODES };
+enum { SC_TAIL = -1, SC_OK = 0, SC_RECORD, SC_REFID, SC_UNPLACED, SC_NO_NM, SC_ANCHOR, SC_AUX, SC_NO_NUM_NM, SC_NO_CIGAR,
+       SC_NEG_POS, SC_NCODES };
 
 const char *scan_msg(int c) {
   static const char *m[SC_NCODES] = {"ok", "malformed BAM record", "refID out of range",
                                      "unplaced read before the end of the placed reads", "no integer NM tag",
                                      "the record walk does not land on the next index anchor (index of another file?)",
-                                     "malformed auxiliary field"};
+                                     "malformed auxiliary field", "no numeric NM tag (types c, C, s, S, i, I or f)",
+                                     "no CIGAR, so no alignment length", "mapped read at a negative position"};
   return c >= 0 && c < SC_NCODES ? m[c] : "unknown";
 }
+
+// codes whose message names the read
+bool scan_names_read(int c) { return c == SC_NO_NM || c == SC_NO_NUM_NM || c == SC_NO_CIGAR || c == SC_NEG_POS; }
 
 struct ScanParams {
   const uint8_t *data;                        // 4-byte aligned, readable 8 bytes past the last segment end
@@ -375,8 +388,9 @@ __device__ __forceinline__ int64_t aligned_length(const uint8_t *d, int64_t cig,
   return end - start;
 }
 
-// NM as an integer: 0 found, SC_NO_NM absent or not of type cCsSiI, SC_AUX malformed
-__device__ int find_nm(const uint8_t *d, int64_t a, int64_t e, int64_t *nm) {
+// The NM field of the auxiliary data [a, e): SC_OK with its type in *ty and, for a fixed-size type, its value's position
+// in *at (the bytes are inside [a, e)); SC_NO_NM absent; SC_AUX malformed (before or at NM).
+__device__ int locate_nm(const uint8_t *d, int64_t a, int64_t e, uint8_t *ty_out, int64_t *at) {
   while (a < e) {
     if (e - a < 3) return SC_AUX;
     const uint8_t t0 = d[a], t1 = d[a + 1], ty = d[a + 2];
@@ -391,7 +405,7 @@ __device__ int find_nm(const uint8_t *d, int64_t a, int64_t e, int64_t *nm) {
         int64_t z = a;
         while (z < e && d[z] != 0) ++z;
         if (z >= e) return SC_AUX;
-        if (is_nm) return SC_NO_NM;
+        if (is_nm) { *ty_out = ty; return SC_OK; }
         a = z + 1;
         continue;
       }
@@ -402,35 +416,87 @@ __device__ int find_nm(const uint8_t *d, int64_t a, int64_t e, int64_t *nm) {
         if (!es) return SC_AUX;
         const int64_t cnt = (int64_t)ld32(d, a + 1);
         if (cnt * es > e - a - 5) return SC_AUX;
-        if (is_nm) return SC_NO_NM;
+        if (is_nm) { *ty_out = ty; return SC_OK; }
         a += 5 + cnt * es;
         continue;
       }
       default: return SC_AUX;
     }
     if (e - a < sz) return SC_AUX;
-    if (is_nm) {
-      int64_t v;
-      switch (ty) {
-        case 'c': v = (int8_t)d[a]; break;
-        case 'C': v = d[a]; break;
-        case 's': v = (int16_t)(d[a] | d[a + 1] << 8); break;
-        case 'S': v = (uint16_t)(d[a] | d[a + 1] << 8); break;
-        case 'i': v = (int32_t)ld32(d, a); break;
-        case 'I': v = (uint32_t)ld32(d, a); break;
-        default: return SC_NO_NM;                                  // 'A' or 'f'
-      }
-      *nm = v;
-      return SC_OK;
-    }
+    if (is_nm) { *ty_out = ty; *at = a; return SC_OK; }
     a += sz;
   }
   return SC_NO_NM;
 }
 
-__device__ __forceinline__ void flush(const ScanParams &q, int ref, unsigned long long *c) {
+// an integer aux value of type cCsSiI at d[a]; false for any other type
+__device__ __forceinline__ bool aux_int(const uint8_t *d, int64_t a, uint8_t ty, int64_t *v) {
+  switch (ty) {
+    case 'c': *v = (int8_t)d[a]; return true;
+    case 'C': *v = d[a]; return true;
+    case 's': *v = (int16_t)(d[a] | d[a + 1] << 8); return true;
+    case 'S': *v = (uint16_t)(d[a] | d[a + 1] << 8); return true;
+    case 'i': *v = (int32_t)ld32(d, a); return true;
+    case 'I': *v = (uint32_t)ld32(d, a); return true;
+    default: return false;
+  }
+}
+
+// NM as an integer: 0 found, SC_NO_NM absent or not of type cCsSiI, SC_AUX malformed
+__device__ int find_nm(const uint8_t *d, int64_t a, int64_t e, int64_t *nm) {
+  uint8_t ty = 0;
+  int64_t at = 0;
+  const int rc = locate_nm(d, a, e, &ty, &at);
+  if (rc) return rc;
+  return aux_int(d, at, ty, nm) ? SC_OK : SC_NO_NM;
+}
+
+// NM as pysam's get_tag gives it to a numeric comparison: an integer type, or the float of type f (widened to double).
+// 0 found, SC_NO_NUM_NM absent or of type A, Z, H or B, SC_AUX malformed.
+__device__ int find_nm_number(const uint8_t *d, int64_t a, int64_t e, double *nm) {
+  uint8_t ty = 0;
+  int64_t at = 0;
+  const int rc = locate_nm(d, a, e, &ty, &at);
+  if (rc) return rc == SC_NO_NM ? SC_NO_NUM_NM : rc;
+  int64_t v;
+  if (aux_int(d, at, ty, &v)) { *nm = (double)v; return SC_OK; }
+  if (ty == 'f') { *nm = (double)__uint_as_float(ld32(d, at)); return SC_OK; }
+  return SC_NO_NUM_NM;
+}
+
+// One record's fields, decoded and bounds-checked by decode_record.
+struct Rec {
+  int32_t ref, pos, l_seq;
+  int mapq, n_cigar, flag;
+  int64_t cig, aux, end;                      // CIGAR and auxiliary data positions, the next record's position
+};
+
+// The record at stream position p of a segment ending at `end`: SC_OK, SC_TAIL at the first unplaced record of the last
+// segment, or the code that stops the walk.
+__device__ __forceinline__ int decode_record(const uint8_t *d, int64_t p, int64_t end, int32_t n_ref, bool last_seg, Rec &r) {
+  if (end - p < 36) return SC_ANCHOR;
+  const int32_t bs = (int32_t)ld32(d, p);
+  if (bs < 32) return SC_RECORD;
+  if (bs > end - p - 4) return SC_ANCHOR;
+  r.ref = (int32_t)ld32(d, p + 4);
+  if (r.ref < -1 || r.ref >= n_ref) return SC_REFID;
+  if (r.ref == -1) return last_seg ? SC_TAIL : SC_UNPLACED;
+  r.pos = (int32_t)ld32(d, p + 8);
+  const uint32_t w3 = ld32(d, p + 12), w4 = ld32(d, p + 16);
+  const int l_name = (int)(w3 & 0xFF);
+  r.mapq = (int)((w3 >> 8) & 0xFF);
+  r.n_cigar = (int)(w4 & 0xFFFF); r.flag = (int)(w4 >> 16);
+  r.l_seq = (int32_t)ld32(d, p + 20);
+  r.end = p + 4 + bs;
+  r.cig = p + 4 + 32 + l_name;
+  r.aux = r.cig + 4ll * r.n_cigar + ((int64_t)r.l_seq + 1) / 2 + r.l_seq;
+  if (l_name < 1 || r.l_seq < 0 || r.aux > r.end) return SC_RECORD;
+  return SC_OK;
+}
+
+__device__ __forceinline__ void flush(unsigned long long *counters, int ref, unsigned long long *c) {
   if (ref >= 0) {
-    unsigned long long *dst = q.counters + (size_t)ref * NCNT;
+    unsigned long long *dst = counters + (size_t)ref * NCNT;
 #pragma unroll
     for (int k = 0; k < NCNT; ++k)
       if (c[k]) atomicAdd(dst + k, c[k]);
@@ -450,42 +516,126 @@ __global__ void __launch_bounds__(SCAN_THREADS) bam_scan_kernel(ScanParams q) {
   for (int k = 0; k < NCNT; ++k) c[k] = 0;
   int cur = -1, code = SC_OK;
   while (pos < end) {
-    if (end - pos < 36) { code = SC_ANCHOR; break; }
-    const int32_t bs = (int32_t)ld32(d, pos);
-    if (bs < 32) { code = SC_RECORD; break; }
-    if (bs > end - pos - 4) { code = SC_ANCHOR; break; }
-    const int32_t ref = (int32_t)ld32(d, pos + 4);
-    if (ref < -1 || ref >= q.n_ref) { code = SC_REFID; break; }
-    if (ref == -1) { if (s != q.nseg - 1) code = SC_UNPLACED; break; }
-    const uint32_t w3 = ld32(d, pos + 12), w4 = ld32(d, pos + 16);
-    const int l_name = (int)(w3 & 0xFF), mapq = (int)((w3 >> 8) & 0xFF);
-    const int n_cigar = (int)(w4 & 0xFFFF), flag = (int)(w4 >> 16);
-    const int32_t l_seq = (int32_t)ld32(d, pos + 20);
-    const int64_t rec = pos + 4, rend = rec + bs;
-    const int64_t cig = rec + 32 + l_name;
-    if (l_name < 1 || l_seq < 0 || cig + 4ll * n_cigar + ((int64_t)l_seq + 1) / 2 + l_seq > rend) { code = SC_RECORD; break; }
-    if (ref != cur) { flush(q, cur, c); cur = ref; }
+    Rec r;
+    const int rc0 = decode_record(d, pos, end, q.n_ref, s == q.nseg - 1, r);
+    if (rc0) { if (rc0 != SC_TAIL) code = rc0; break; }
+    const int flag = r.flag, l_seq = r.l_seq;
+    if (r.ref != cur) { flush(q.counters, cur, c); cur = r.ref; }
     c[0]++;
     if (flag & 0x4) {
     } else if (flag & 0x400) c[1]++;
     else if (flag & 0x900) c[2]++;
-    else if ((flag & 0x200) || mapq < q.min_qc) c[3]++;
+    else if ((flag & 0x200) || r.mapq < q.min_qc) c[3]++;
     else {
-      const int64_t qal = aligned_length(d, cig, n_cigar, l_seq);
+      const int64_t qal = aligned_length(d, r.cig, r.n_cigar, l_seq);
       if ((double)qal < q.min_align * (double)l_seq) c[4]++;
       else {
         int64_t nm = 0;
-        const int rc = find_nm(d, cig + 4ll * n_cigar + ((int64_t)l_seq + 1) / 2 + l_seq, rend, &nm);
+        const int rc = find_nm(d, r.aux, r.end, &nm);
         if (rc) { code = rc; break; }
         if ((double)nm > q.max_edit * (double)l_seq) c[5]++;
         else if (!q.all_reads && !(flag & 0x2)) c[6]++;
         else { c[7]++; c[8] += (unsigned long long)qal; }
       }
     }
-    pos = rend;
+    pos = r.end;
   }
   if (code) atomicMin(q.err, (unsigned long long)pos << 8 | (unsigned long long)code);
-  flush(q, cur, c);
+  flush(q.counters, cur, c);
+}
+
+struct WinParams {
+  const uint8_t *data;                        // as ScanParams
+  const int64_t *seg_start, *seg_end; int64_t nseg;
+  int32_t n_ref, all_reads; double min_align, max_edit;
+  const int64_t *ref_len;                     // header lengths
+  const int64_t *win_off;                     // n_ref + 1: reference r's windows are windows[win_off[r] .. win_off[r + 1])
+  int64_t W;
+  unsigned long long *counters;               // n_ref x NCNT; the ninth is the clipped covered bases
+  unsigned long long *windows;                // per window: the sum of the depth over it
+  unsigned long long *touched;                // [0] smallest window written, [1] largest + 1
+  unsigned long long *err;
+};
+
+// reference span of the CIGAR: M, D, N, =, X (pysam's reference_length, coverageWindows' `alen`)
+__device__ __forceinline__ int64_t reference_span(const uint8_t *d, int64_t cig, int nc) {
+  int64_t s = 0;
+  for (int k = 0; k < nc; ++k) {
+    const uint32_t c = ld32(d, cig + 4ll * k), o = c & 15u;
+    if (o == 0 || o == 2 || o == 3 || o == 7 || o == 8) s += c >> 4;
+  }
+  return s;
+}
+
+__global__ void __launch_bounds__(SCAN_THREADS) bam_window_kernel(WinParams q) {
+  const int64_t s = (int64_t)blockIdx.x * SCAN_THREADS + threadIdx.x;
+  if (s >= q.nseg) return;
+  const uint8_t *d = q.data;
+  int64_t pos = q.seg_start[s];
+  const int64_t end = q.seg_end[s];
+  unsigned long long c[NCNT];
+#pragma unroll
+  for (int k = 0; k < NCNT; ++k) c[k] = 0;
+  int cur = -1, code = SC_OK;
+  int64_t L = 0, off = 0, nwin = 0;
+  int64_t wi = -1;                                                 // cached window (global index) and its partial sum
+  unsigned long long wsum = 0;
+  unsigned long long lo = ~0ull, hi = 0;
+  const int64_t W = q.W;
+  while (pos < end) {
+    Rec r;
+    const int rc0 = decode_record(d, pos, end, q.n_ref, s == q.nseg - 1, r);
+    if (rc0) { if (rc0 != SC_TAIL) code = rc0; break; }
+    const int flag = r.flag;
+    const double l_seq = (double)r.l_seq;
+    if (r.ref != cur) {
+      flush(q.counters, cur, c);
+      cur = r.ref; L = q.ref_len[cur]; off = q.win_off[cur]; nwin = q.win_off[cur + 1] - off;
+    }
+    const int64_t alen = reference_span(d, r.cig, r.n_cigar);
+    const int64_t rp = r.pos;
+    // fetch(ref, 0, L) yields the records overlapping [0, L): end = pos + span, or pos + 1 when unmapped or empty
+    const int64_t fend = rp + ((flag & 0x4) || alen == 0 ? 1 : alen);
+    if (rp < L && fend > 0) {
+      c[0]++;
+      if (flag & 0x4) {
+      } else if (flag & 0x400) c[1]++;
+      else if (flag & 0x100) c[2]++;                               // supplementary reads fall through
+      else if (flag & 0x200) c[3]++;                               // no mapping-quality threshold
+      else if (r.n_cigar == 0) { code = SC_NO_CIGAR; break; }
+      else if ((double)alen < q.min_align * l_seq) c[4]++;
+      else {
+        double nm = 0.0;
+        const int rc = find_nm_number(d, r.aux, r.end, &nm);
+        if (rc) { code = rc; break; }
+        if (nm > q.max_edit * l_seq) c[5]++;
+        else if (!q.all_reads && !(flag & 0x2)) c[6]++;
+        else if (rp < 0) { code = SC_NEG_POS; break; }
+        else {
+          c[7]++;
+          const int64_t b = min(rp + alen, L);                     // numpy's slice clips at the reference end
+          if (b > rp) {
+            c[8] += (unsigned long long)(b - rp);
+            const int64_t klast = min((b - 1) / W, nwin - 1);
+            for (int64_t k = rp / W; k <= klast; ++k) {
+              const int64_t g = off + k;
+              if (g != wi) {
+                if (wsum) atomicAdd(q.windows + wi, wsum);
+                wi = g; wsum = 0;
+                lo = min(lo, (unsigned long long)g); hi = max(hi, (unsigned long long)g + 1);
+              }
+              wsum += (unsigned long long)(min(b, (k + 1) * W) - max(rp, k * W));
+            }
+          }
+        }
+      }
+    }
+    pos = r.end;
+  }
+  if (code) atomicMin(q.err, (unsigned long long)pos << 8 | (unsigned long long)code);
+  flush(q.counters, cur, c);
+  if (wsum) atomicAdd(q.windows + wi, wsum);
+  if (hi) { atomicMin(q.touched, lo); atomicMax(q.touched + 1, hi); }
 }
 
 const uint32_t *x2n_table() {
@@ -574,6 +724,69 @@ int inflate_batch(ckm_engine *e, const char *fn, const uint8_t *comp, int64_t co
   return CKM_OK;
 }
 
+// check_blocks, and every segment inside the batch's decompressed range
+int check_batch(const char *fn, int64_t comp_base, int64_t comp_len, const ckm_bgzf_block *blocks, int64_t nblocks,
+                const int64_t *seg_start, const int64_t *seg_end, int64_t nseg, std::vector<int64_t> &uoff) {
+  int rc;
+  if ((rc = check_blocks(fn, comp_base, comp_len, blocks, nblocks, uoff))) return rc;
+  const int64_t total = uoff.back();
+  for (int64_t s = 0; s < nseg; ++s)
+    if (seg_start[s] < 0 || seg_start[s] > seg_end[s] || seg_end[s] > total) {
+      char msg[160];
+      std::snprintf(msg, sizeof msg, "%s: a segment does not lie in the batch's decompressed range", fn);
+      set_error(msg); return CKM_EINVAL;
+    }
+  return CKM_OK;
+}
+
+// Inflates the batch into dout and uploads the segments into dseg (starts, then ends).  kernel_ms_out[0]: the inflate.
+int inflate_and_upload(ckm_engine *e, const char *fn, const uint8_t *comp, int64_t comp_base, int64_t comp_len,
+                       const ckm_bgzf_block *blocks, int64_t nblocks, const std::vector<int64_t> &uoff,
+                       const int64_t *seg_start, const int64_t *seg_end, int64_t nseg, DevBuf &dout, DevBuf &dseg,
+                       float *kernel_ms_out, int64_t *err_offset_out) {
+  cudaStream_t st = e->stream;
+  int64_t bad_block = -1;
+  float ms_inflate = 0.0f;
+  int rc;
+  if ((rc = inflate_batch(e, fn, comp, comp_base, comp_len, blocks, nblocks, uoff, dout, &bad_block, &ms_inflate))) {
+    if (err_offset_out && bad_block >= 0) *err_offset_out = blocks[bad_block].coffset;
+    return rc;
+  }
+  if (kernel_ms_out) kernel_ms_out[0] = ms_inflate;
+  if ((rc = dseg.alloc(sizeof(int64_t) * 2 * (size_t)std::max<int64_t>(nseg, 1)))) return rc;
+  if (nseg) {
+    CKM_CUDA(cudaMemcpyAsync(dseg.p, seg_start, sizeof(int64_t) * (size_t)nseg, cudaMemcpyHostToDevice, st));
+    CKM_CUDA(cudaMemcpyAsync(dseg.as<int64_t>() + nseg, seg_end, sizeof(int64_t) * (size_t)nseg, cudaMemcpyHostToDevice, st));
+  }
+  return CKM_OK;
+}
+
+// CKM_EFORMAT for a walk's error word (record position << 8 | code): the record's virtual offset and, for the codes
+// that concern one read, its name.
+int scan_error(const char *fn, unsigned long long err, const ckm_bgzf_block *blocks, int64_t nblocks,
+               const std::vector<int64_t> &uoff, DevBuf &dout, int64_t *err_offset_out) {
+  const int64_t total = uoff.back();
+  const int code = (int)(err & 0xFF);
+  const int64_t pos = (int64_t)(err >> 8);
+  const int64_t b = std::upper_bound(uoff.begin(), uoff.end() - 1, pos) - uoff.begin() - 1;   // block holding pos
+  const int64_t voff = b >= 0 && b < nblocks ? (blocks[b].coffset << 16 | (pos - uoff[b])) : -1;
+  std::string name;
+  if (scan_names_read(code)) {
+    char rec[300];
+    const int64_t nb = std::min<int64_t>((int64_t)sizeof rec, total + 8 - pos);
+    CKM_CUDA(cudaMemcpy(rec, dout.as<uint8_t>() + pos, (size_t)nb, cudaMemcpyDeviceToHost));
+    const int l = (uint8_t)rec[12];
+    for (int i = 0; i < l - 1 && 36 + i < nb && rec[36 + i]; ++i) name += rec[36 + i];
+  }
+  char msg[512];
+  std::snprintf(msg, sizeof msg, "%s: record at virtual offset %lld (block at file offset %lld + %lld): %s%s%s", fn,
+                (long long)voff, (long long)(b >= 0 && b < nblocks ? blocks[b].coffset : -1), (long long)(b >= 0 ? pos - uoff[b] : -1),
+                scan_msg(code), name.empty() ? "" : " in read ", name.c_str());
+  set_error(msg);
+  if (err_offset_out) *err_offset_out = voff;
+  return CKM_EFORMAT;
+}
+
 }  // namespace
 
 extern "C" {
@@ -652,32 +865,18 @@ int ckm_bam_coverage(ckm_engine *e, const uint8_t *comp, int64_t comp_base, int6
   if (err_offset_out) *err_offset_out = -1;
   std::vector<int64_t> uoff;
   int rc;
-  if ((rc = check_blocks("ckm_bam_coverage", comp_base, comp_len, blocks, nblocks, uoff))) return rc;
-  const int64_t total = uoff.back();
-  for (int64_t s = 0; s < nseg; ++s)
-    if (seg_start[s] < 0 || seg_start[s] > seg_end[s] || seg_end[s] > total) {
-      set_error("ckm_bam_coverage: a segment does not lie in the batch's decompressed range"); return CKM_EINVAL;
-    }
+  if ((rc = check_batch("ckm_bam_coverage", comp_base, comp_len, blocks, nblocks, seg_start, seg_end, nseg, uoff))) return rc;
   cudaSetDevice(e->device);
   PoolScope pool_scope(e);
   cudaStream_t st = e->stream;
-  DevBuf dout;
-  int64_t bad_block = -1;
-  float ms_inflate = 0.0f;
-  if ((rc = inflate_batch(e, "ckm_bam_coverage", comp, comp_base, comp_len, blocks, nblocks, uoff, dout, &bad_block, &ms_inflate))) {
-    if (err_offset_out && bad_block >= 0) *err_offset_out = blocks[bad_block].coffset;
+  DevBuf dout, dseg;
+  if ((rc = inflate_and_upload(e, "ckm_bam_coverage", comp, comp_base, comp_len, blocks, nblocks, uoff, seg_start, seg_end, nseg,
+                               dout, dseg, kernel_ms_out, err_offset_out)))
     return rc;
-  }
-  if (kernel_ms_out) kernel_ms_out[0] = ms_inflate;
-  DevBuf dseg, dcnt, derr;
+  DevBuf dcnt, derr;
   const size_t ncnt = (size_t)n_ref * NCNT;
-  if ((rc = dseg.alloc(sizeof(int64_t) * 2 * (size_t)std::max<int64_t>(nseg, 1))) || (rc = dcnt.alloc(sizeof(int64_t) * std::max<size_t>(ncnt, 1))) ||
-      (rc = derr.alloc(sizeof(unsigned long long))))
+  if ((rc = dcnt.alloc(sizeof(int64_t) * std::max<size_t>(ncnt, 1))) || (rc = derr.alloc(sizeof(unsigned long long))))
     return rc;
-  if (nseg) {
-    CKM_CUDA(cudaMemcpyAsync(dseg.p, seg_start, sizeof(int64_t) * (size_t)nseg, cudaMemcpyHostToDevice, st));
-    CKM_CUDA(cudaMemcpyAsync(dseg.as<int64_t>() + nseg, seg_end, sizeof(int64_t) * (size_t)nseg, cudaMemcpyHostToDevice, st));
-  }
   if (ncnt) CKM_CUDA(cudaMemsetAsync(dcnt.p, 0, sizeof(int64_t) * ncnt, st));
   CKM_CUDA(cudaMemsetAsync(derr.p, 0xFF, sizeof(unsigned long long), st));
   ScanParams q;
@@ -699,28 +898,110 @@ int ckm_bam_coverage(ckm_engine *e, const uint8_t *comp, int64_t comp_base, int6
   float ms_scan = 0.0f;
   CKM_CUDA(cudaEventElapsedTime(&ms_scan, e->ev[0], e->ev[1]));
   if (kernel_ms_out) kernel_ms_out[1] = ms_scan;
-  if (err != ~0ull) {
-    const int code = (int)(err & 0xFF);
-    const int64_t pos = (int64_t)(err >> 8);
-    const int64_t b = std::upper_bound(uoff.begin(), uoff.end() - 1, pos) - uoff.begin() - 1;   // block holding pos
-    const int64_t voff = b >= 0 && b < nblocks ? (blocks[b].coffset << 16 | (pos - uoff[b])) : -1;
-    std::string name;
-    if (code == SC_NO_NM) {
-      char rec[300];
-      const int64_t nb = std::min<int64_t>((int64_t)sizeof rec, total + 8 - pos);
-      CKM_CUDA(cudaMemcpy(rec, dout.as<uint8_t>() + pos, (size_t)nb, cudaMemcpyDeviceToHost));
-      const int l = (uint8_t)rec[12];
-      for (int i = 0; i < l - 1 && 36 + i < nb && rec[36 + i]; ++i) name += rec[36 + i];
-    }
-    char msg[512];
-    std::snprintf(msg, sizeof msg, "ckm_bam_coverage: record at virtual offset %lld (block at file offset %lld + %lld): %s%s%s",
-                  (long long)voff, (long long)(b >= 0 && b < nblocks ? blocks[b].coffset : -1), (long long)(b >= 0 ? pos - uoff[b] : -1),
-                  scan_msg(code), name.empty() ? "" : " in read ", name.c_str());
-    set_error(msg);
-    if (err_offset_out) *err_offset_out = voff;
-    return CKM_EFORMAT;
-  }
+  if (err != ~0ull) return scan_error("ckm_bam_coverage", err, blocks, nblocks, uoff, dout, err_offset_out);
   for (size_t k = 0; k < ncnt; ++k) counters[k] += cnt[k];
+  return CKM_OK;
+}
+
+int ckm_bam_windows(ckm_engine *e, const uint8_t *comp, int64_t comp_base, int64_t comp_len, const ckm_bgzf_block *blocks,
+                    int64_t nblocks, const int64_t *seg_start, const int64_t *seg_end, int64_t nseg, int32_t n_ref,
+                    const ckm_bam_filter *filter, const int64_t *ref_len, int64_t window_size, const int64_t *win_off,
+                    int64_t *counters, int64_t *windows, float *kernel_ms_out, int64_t *err_offset_out) {
+  if (!e || comp_len < 0 || (comp_len > 0 && !comp) || nblocks < 0 || (nblocks > 0 && !blocks) || nseg < 0 ||
+      (nseg > 0 && (!seg_start || !seg_end)) || n_ref < 0 || !filter || (n_ref > 0 && (!counters || !ref_len)) || !win_off) {
+    set_error("ckm_bam_windows: bad argument"); return CKM_EINVAL;
+  }
+  if (kernel_ms_out) kernel_ms_out[0] = kernel_ms_out[1] = 0.0f;
+  if (err_offset_out) *err_offset_out = -1;
+  char msg[320];
+  if (window_size <= 0) {
+    std::snprintf(msg, sizeof msg, "ckm_bam_windows: window size %lld; it must be at least 1", (long long)window_size);
+    set_error(msg); return CKM_EINVAL;
+  }
+  if (win_off[0] != 0) { set_error("ckm_bam_windows: win_off[0] must be 0"); return CKM_EINVAL; }
+  for (int32_t r = 0; r < n_ref; ++r) {
+    if (ref_len[r] <= 0) {
+      std::snprintf(msg, sizeof msg, "ckm_bam_windows: reference %d has length %lld; coverage per base needs a length of at "
+                    "least 1", r, (long long)ref_len[r]);
+      set_error(msg); return CKM_EINVAL;
+    }
+    if (win_off[r + 1] - win_off[r] != (ref_len[r] - 1) / window_size) {
+      std::snprintf(msg, sizeof msg, "ckm_bam_windows: reference %d has %lld windows in win_off, (length - 1) / window size "
+                    "is %lld", r, (long long)(win_off[r + 1] - win_off[r]), (long long)((ref_len[r] - 1) / window_size));
+      set_error(msg); return CKM_EINVAL;
+    }
+  }
+  const int64_t nwin = win_off[n_ref];
+  if (nwin > 0 && !windows) { set_error("ckm_bam_windows: bad argument"); return CKM_EINVAL; }
+  std::vector<int64_t> uoff;
+  int rc;
+  if ((rc = check_batch("ckm_bam_windows", comp_base, comp_len, blocks, nblocks, seg_start, seg_end, nseg, uoff))) return rc;
+  cudaSetDevice(e->device);
+  PoolScope pool_scope(e);
+  cudaStream_t st = e->stream;
+  // the window array first: it is the one buffer whose size the caller chooses through W
+  DevBuf dwin;
+  size_t free_b = 0, total_b = 0;
+  CKM_CUDA(cudaMemGetInfo(&free_b, &total_b));
+  const double need = 8.0 * (double)nwin;
+  if (need > (double)free_b || dwin.alloc(sizeof(int64_t) * (size_t)std::max<int64_t>(nwin, 1))) {
+    cudaGetLastError();
+    if (need <= (double)free_b) CKM_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    // the smallest W whose window array fits in the free memory (sum of (len - 1) / W falls as W grows)
+    auto windows_at = [&](int64_t w) { int64_t t = 0; for (int32_t r = 0; r < n_ref; ++r) t += (ref_len[r] - 1) / w; return t; };
+    const int64_t cap = (int64_t)(free_b / 8);
+    int64_t lo_w = window_size, hi_w = window_size;
+    while (windows_at(hi_w) > cap && hi_w < (int64_t(1) << 40)) hi_w *= 2;
+    while (lo_w < hi_w) { const int64_t m = lo_w + (hi_w - lo_w) / 2; if (windows_at(m) > cap) lo_w = m + 1; else hi_w = m; }
+    std::snprintf(msg, sizeof msg, "ckm_bam_windows: %lld windows of %lld bp need %.1f MiB of device memory, %.1f MiB are "
+                  "free; the smallest window size that fits is %lld", (long long)nwin, (long long)window_size,
+                  need / 1048576.0, (double)free_b / 1048576.0, (long long)lo_w);
+    set_error(msg); return CKM_ENOMEM;
+  }
+  DevBuf dout, dseg;
+  if ((rc = inflate_and_upload(e, "ckm_bam_windows", comp, comp_base, comp_len, blocks, nblocks, uoff, seg_start, seg_end, nseg,
+                               dout, dseg, kernel_ms_out, err_offset_out)))
+    return rc;
+  DevBuf dcnt, dmeta, dlen;
+  const size_t ncnt = (size_t)n_ref * NCNT;
+  if ((rc = dcnt.alloc(sizeof(int64_t) * std::max<size_t>(ncnt, 1))) || (rc = dmeta.alloc(3 * sizeof(unsigned long long))) ||
+      (rc = dlen.alloc(sizeof(int64_t) * (2 * (size_t)n_ref + 1))))
+    return rc;
+  if (ncnt) CKM_CUDA(cudaMemsetAsync(dcnt.p, 0, sizeof(int64_t) * ncnt, st));
+  if (nwin) CKM_CUDA(cudaMemsetAsync(dwin.p, 0, sizeof(int64_t) * (size_t)nwin, st));
+  const unsigned long long meta0[3] = {~0ull, 0ull, ~0ull};        // touched [lo, hi), error
+  CKM_CUDA(cudaMemcpyAsync(dmeta.p, meta0, sizeof meta0, cudaMemcpyHostToDevice, st));
+  if (n_ref) CKM_CUDA(cudaMemcpyAsync(dlen.p, ref_len, sizeof(int64_t) * (size_t)n_ref, cudaMemcpyHostToDevice, st));
+  CKM_CUDA(cudaMemcpyAsync(dlen.as<int64_t>() + n_ref, win_off, sizeof(int64_t) * ((size_t)n_ref + 1), cudaMemcpyHostToDevice, st));
+  WinParams q;
+  q.data = dout.as<uint8_t>(); q.seg_start = dseg.as<int64_t>(); q.seg_end = dseg.as<int64_t>() + nseg; q.nseg = nseg;
+  q.n_ref = n_ref; q.all_reads = filter->all_reads; q.min_align = filter->min_align; q.max_edit = filter->max_edit;
+  q.ref_len = dlen.as<int64_t>(); q.win_off = dlen.as<int64_t>() + n_ref; q.W = window_size;
+  q.counters = dcnt.as<unsigned long long>(); q.windows = dwin.as<unsigned long long>();
+  q.touched = dmeta.as<unsigned long long>(); q.err = dmeta.as<unsigned long long>() + 2;
+  CKM_CUDA(cudaEventRecord(e->ev[0], st));
+  if (nseg) {
+    bam_window_kernel<<<(unsigned)((nseg + SCAN_THREADS - 1) / SCAN_THREADS), SCAN_THREADS, 0, st>>>(q);
+    CKM_CUDA(cudaGetLastError());
+  }
+  CKM_CUDA(cudaEventRecord(e->ev[1], st));
+  unsigned long long meta[3];
+  std::vector<int64_t> cnt(ncnt);
+  CKM_CUDA(cudaMemcpyAsync(meta, dmeta.p, sizeof meta, cudaMemcpyDeviceToHost, st));
+  if (ncnt) CKM_CUDA(cudaMemcpyAsync(cnt.data(), dcnt.p, sizeof(int64_t) * ncnt, cudaMemcpyDeviceToHost, st));
+  CKM_CUDA(cudaStreamSynchronize(st));
+  float ms_scan = 0.0f;
+  CKM_CUDA(cudaEventElapsedTime(&ms_scan, e->ev[0], e->ev[1]));
+  if (kernel_ms_out) kernel_ms_out[1] = ms_scan;
+  if (meta[2] != ~0ull) return scan_error("ckm_bam_windows", meta[2], blocks, nblocks, uoff, dout, err_offset_out);
+  for (size_t k = 0; k < ncnt; ++k) counters[k] += cnt[k];
+  // only the windows this batch wrote come back: a batch covers a run of references, not the whole array
+  if (meta[1] > meta[0]) {
+    const size_t lo = (size_t)meta[0], n = (size_t)(meta[1] - meta[0]);
+    std::vector<int64_t> w(n);
+    CKM_CUDA(cudaMemcpy(w.data(), dwin.as<int64_t>() + lo, sizeof(int64_t) * n, cudaMemcpyDeviceToHost));
+    for (size_t k = 0; k < n; ++k) windows[lo + k] += w[k];
+  }
   return CKM_OK;
 }
 

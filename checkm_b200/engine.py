@@ -309,6 +309,36 @@ class Engine:
                                           counters.ctypes.data if n_ref else None, ms, C.byref(err)))
         return float(ms[0]), float(ms[1])
 
+    def bam_windows(self, comp, blocks, seg_start, seg_end, ref_len, window_size, win_off, counters, windows, comp_base=0,
+                    all_reads=False, min_align=0.98, max_edit=0.02):
+        """One batch of a BAM (ckm_bam_windows): blocks inflated, the segments walked with coverageWindows' rule, the nine
+        counters of every reference added to `counters` (n_ref x 9 int64; the ninth is the covered bases) and each
+        window's depth sum to `windows` (int64; reference r owns windows[win_off[r]:win_off[r + 1]]).  Returns the
+        inflate and window kernels' durations in ms."""
+        comp = np.ascontiguousarray(np.frombuffer(comp, dtype=np.uint8) if not isinstance(comp, np.ndarray) else comp)
+        blocks = np.ascontiguousarray(blocks)
+        seg_start = np.ascontiguousarray(seg_start, dtype=np.int64)
+        seg_end = np.ascontiguousarray(seg_end, dtype=np.int64)
+        ref_len = np.ascontiguousarray(ref_len, dtype=np.int64)
+        win_off = np.ascontiguousarray(win_off, dtype=np.int64)
+        n_ref = len(ref_len)
+        if counters.dtype != np.int64 or counters.shape != (n_ref, 9) or not counters.flags.c_contiguous:
+            raise ValueError("bam_windows: counters must be a C-contiguous n_ref x 9 int64 array")
+        if win_off.shape != (n_ref + 1,):
+            raise ValueError("bam_windows: win_off must hold n_ref + 1 offsets")
+        if windows.dtype != np.int64 or windows.ndim != 1 or not windows.flags.c_contiguous or windows.size < win_off[-1]:
+            raise ValueError("bam_windows: windows must be a C-contiguous int64 array of win_off[-1] values")
+        filt = _lib.BamFilter(int(bool(all_reads)), 0, float(min_align), float(max_edit))
+        ms = (C.c_float * 2)()
+        err = C.c_int64()
+        check(_lib.lib().ckm_bam_windows(self._h, comp.ctypes.data if comp.size else None, int(comp_base), comp.size,
+                                         blocks.ctypes.data if len(blocks) else None, len(blocks), seg_start.ctypes.data,
+                                         seg_end.ctypes.data, len(seg_start), n_ref, C.byref(filt),
+                                         ref_len.ctypes.data if n_ref else None, int(window_size), win_off.ctypes.data,
+                                         counters.ctypes.data if n_ref else None, windows.ctypes.data if windows.size else None,
+                                         ms, C.byref(err)))
+        return float(ms[0]), float(ms[1])
+
     def close(self):
         if self._h:
             _lib.lib().ckm_destroy(self._h)

@@ -382,6 +382,24 @@ typedef struct {
 int  ckm_bam_coverage(ckm_engine *e, const uint8_t *comp, int64_t comp_base, int64_t comp_len, const ckm_bgzf_block *blocks,
                       int64_t nblocks, const int64_t *seg_start, const int64_t *seg_end, int64_t nseg, int32_t n_ref,
                       const ckm_bam_filter *filter, int64_t *counters, float *kernel_ms_out, int64_t *err_offset_out);
+/* Read depth per window (`checkm gc_bias_plot`, coverageWindows.py:55-79) for one batch, cut and walked as in
+ * ckm_bam_coverage.  A record of reference r counts only if fetch(r, 0, ref_len[r]) yields it: pos < ref_len[r] and
+ * end > 0, end = pos + reference span of the CIGAR (pos + 1 for an unmapped read or an empty span).  The classification is
+ * coverageWindows': secondary is 0x100 only (supplementary reads go on), QC is 0x200 only (filter->min_qc is ignored), the
+ * alignment length is the CIGAR's reference span (M, D, N, =, X) against filter->min_align * l_seq, and NM may be of any
+ * integer type or f.  A mapped read adds 1 to the depth of every base of [pos, min(pos + span, ref_len[r])).
+ * window_size W >= 1 and every ref_len >= 1, else CKM_EINVAL.  win_off (n_ref + 1, win_off[0] = 0): reference r owns
+ * windows[win_off[r] .. win_off[r + 1]), which must number (ref_len[r] - 1) / W; window k covers [k W, (k + 1) W).
+ * counters (n_ref x 9 int64) and windows (win_off[n_ref] int64) are added to: the counters in ckm_bam_coverage's order,
+ * the ninth being the bases covered (the sum of the depth over the reference), and each window's sum of the depth.
+ * CKM_EFORMAT as ckm_bam_coverage, and also, naming the read, for a read that reaches the alignment-length test without a
+ * CIGAR, one that reaches the edit-distance test without an NM tag of a numeric type, and a mapped read at pos < 0.
+ * CKM_ENOMEM when 8 bytes per window do not fit in free device memory; the message names the smallest W that fits.
+ * kernel_ms_out (optional, 2 floats): the inflate and the window kernel by CUDA events. */
+int  ckm_bam_windows(ckm_engine *e, const uint8_t *comp, int64_t comp_base, int64_t comp_len, const ckm_bgzf_block *blocks,
+                     int64_t nblocks, const int64_t *seg_start, const int64_t *seg_end, int64_t nseg, int32_t n_ref,
+                     const ckm_bam_filter *filter, const int64_t *ref_len, int64_t window_size, const int64_t *win_off,
+                     int64_t *counters, int64_t *windows, float *kernel_ms_out, int64_t *err_offset_out);
 
 #ifdef __cplusplus
 }
