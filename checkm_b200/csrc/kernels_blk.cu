@@ -1,19 +1,21 @@
 // kernels_blk.cu -- lane-blocked (register-resident) versions of the Forward filter, the region finder and the
-// envelope rescoring for models with M <= 1024 (classes Q = 2,4,8 in registers; 16,32 with transitions in shared
-// memory).  Same mathematics as kernels_filters.cu / kernels_domdef.cu; one row costs ~20 warp shuffles instead of ~20
-// per 32 model positions.  Longer models keep using the chunked kernels.
+// envelope rescoring for models with M <= 1024 (the classes of BLK_Q in stages.hpp; from Q = 12 on the transitions sit in
+// shared memory).  Same mathematics as kernels_filters.cu / kernels_domdef.cu, whose verdicts and envelope tail they share
+// (filter_common.cuh, domdef_common.cuh); one row costs ~20 warp shuffles instead of ~20 per 32 model positions.  Longer
+// models keep using the chunked kernels.
 #include "engine.hpp"
 #include "device_utils.cuh"
 #include "stages.hpp"
 #include "fwdback.cuh"
 #include "fwdback_blk.cuh"
 #include "domdef_common.cuh"
+#include "filter_common.cuh"
 
 namespace ckm {
 
 constexpr int BLK_WARPS = 4;
 
-template <int Q> __host__ __device__ constexpr size_t blk_tsm_bytes() { return (size_t)Q * 32 * 2 * sizeof(float4); }
+__host__ __device__ constexpr size_t blk_tsm_bytes(int Q) { return (size_t)Q * 32 * 2 * sizeof(float4); }
 
 // ------------------------------------------------------------------------------------------------
 // Forward filter
@@ -32,18 +34,7 @@ __global__ void __launch_bounds__(BLK_WARPS * 32) fwd2_kernel(FilterParams p) {
     BlkModel<Q, TSMEM> bm;
     blk_model_load<Q, TSMEM>(bm, ms, p.tfb, p.rfb, tsm, lane);
     const float fsc = forward_blk<Q, TSMEM, false>(bm, p.res + p.off[s], L, make_specials(L, true), nullptr, nullptr);
-    cd.fwdsc = fsc;
-    const float seq_score = __fdiv_rn(__fsub_rn(fsc, cd.filtersc), 0.69314718055994529f);
-    const double P = exp_surv((double)seq_score, (double)ms.evparam[4], (double)ms.evparam[5]);
-    cd.P = P;
-    if (lane == 0) {
-      if (p.dense_fwd != nullptr) p.dense_fwd[(int64_t)p.model_slot[cd.model] * p.nseq + s] = fsc;
-      if (P <= p.F3) {
-        const int pos = atomicAdd(p.out_count, 1);
-        if (pos < p.out_cap) p.out[pos] = cd;
-        if (p.dense_passed != nullptr) atomicOr_u8(p.dense_passed, (int64_t)p.model_slot[cd.model] * p.nseq + s, 8);
-      }
-    }
+    fwd_verdict(p, cd, fsc, ms, lane);
   }
 }
 
@@ -78,12 +69,47 @@ __global__ void __launch_bounds__(BLK_WARPS * 32) regions2_kernel(DomdefParams p
 // ------------------------------------------------------------------------------------------------
 // Envelope rescoring in the blocked layout
 // ------------------------------------------------------------------------------------------------
+// the traceback's view of the OA matrix: position k lives at q = (k-1) % Q of lane (k-1) / Q
+template <int Q> struct BlockedLayout {
+  const float *F; const float4 *tfb; int M;     // tfb: the model's lane-blocked transitions
+  static __device__ __forceinline__ int at(int k) { return ((k - 1) % Q) * 32 + (k - 1) / Q; }
+  __device__ __forceinline__ float cell(int row, int plane, int k) const { return F[((int64_t)row * 3 + plane) * (Q * 32) + at(k)]; }
+  __device__ __forceinline__ float4 t0(int k) const { return __ldg(tfb + at(k) * 2); }
+  __device__ __forceinline__ float4 t1(int k) const { return __ldg(tfb + at(k) * 2 + 1); }
+  // The walk runs once per domain, but its shape steers the register allocation of the whole kernel: up to Q = 12 one fully
+  // unrolled pass over M and D, beyond that two passes unrolled by 4 (ptxas -v: fewest registers and spill bytes per class).
+  __device__ __forceinline__ void row_best(int row, int lane, float &bm, int &bk, float &bd, int &bdk) const {
+    const float *dpc = F + (int64_t)row * 3 * (Q * 32) + lane;
+    if constexpr (Q <= 12) {
+#pragma unroll
+      for (int q = 0; q < Q; ++q) {
+        const int kk = lane * Q + q + 1;
+        if (kk <= M) {
+          const float v = dpc[q * 32]; if (v >= bm) { bm = v; bk = kk; }
+          const float w = dpc[(Q + q) * 32]; if (w > bd) { bd = w; bdk = kk; }
+        }
+      }
+    } else {
+#pragma unroll 4
+      for (int q = 0; q < Q; ++q) {
+        const int kk = lane * Q + q + 1;
+        if (kk <= M) { const float v = dpc[q * 32]; if (v >= bm) { bm = v; bk = kk; } }
+      }
+#pragma unroll 4
+      for (int q = 0; q < Q; ++q) {
+        const int kk = lane * Q + q + 1;
+        if (kk <= M) { const float w = dpc[(Q + q) * 32]; if (w > bd) { bd = w; bdk = kk; } }
+      }
+    }
+  }
+};
+
 template <int Q, bool TSMEM>
 __global__ void __launch_bounds__(BLK_WARPS * 32) envelope2_kernel(DomdefParams p) {
   extern __shared__ __align__(16) uint8_t bsm[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   float4 *tsm = reinterpret_cast<float4 *>(bsm) + (size_t)warp * Q * 32 * 2;
-  float *null2 = reinterpret_cast<float *>(bsm + (TSMEM ? BLK_WARPS * blk_tsm_bytes<Q>() : 0)) + warp * 32;
+  float *null2 = reinterpret_cast<float *>(bsm + (TSMEM ? BLK_WARPS * blk_tsm_bytes(Q) : 0)) + warp * 32;
   constexpr int QW = Q * 32;
   for (int idx = p.env_begin + blockIdx.x * BLK_WARPS + warp; idx < p.env_end; idx += gridDim.x * BLK_WARPS) {
     const int ei = p.env_order[idx];
@@ -130,29 +156,13 @@ __global__ void __launch_bounds__(BLK_WARPS * 32) envelope2_kernel(DomdefParams 
         ein[q] = (r == 1) ? pi : ein[q] + pi;
       }
     }
-    for (int r = lane; r <= Ld; r += 32) {
-      float pn = 0.f, pj = 0.f, pc = 0.f;
-      if (r >= 1) {
-        const float *f0 = xf + (int64_t)(r - 1) * X_NX, *b1 = xb + (int64_t)r * X_NX;
-        pn = f0[X_N] * b1[X_N] * sp.nloop * scaleproduct;
-        pj = f0[X_J] * b1[X_J] * sp.nloop * scaleproduct;
-        pc = f0[X_C] * b1[X_C] * sp.nloop * scaleproduct;
-      }
-      pps[r * 3 + 0] = pn; pps[r * 3 + 1] = pj; pps[r * 3 + 2] = pc;
-    }
-    __syncwarp();
+    special_posteriors(sp, xf, xb, scaleproduct, pps, Ld, lane);
     const bool range_err = isinf(scaleproduct);
     if (!range_err && !env.null2_done) {
-      float xn = 0.f, xc = 0.f, xj = 0.f;
-      if (lane == 0) {
-        xn = pps[3 + 0]; xj = pps[3 + 1]; xc = pps[3 + 2];
-        for (int r = 2; r <= Ld; ++r) { xn += pps[r * 3 + 0]; xj += pps[r * 3 + 1]; xc += pps[r * 3 + 2]; }
-      }
       const float norm = __fdiv_rn(1.0f, (float)Ld);
+      const float xfactor = special_xfactor(pps, Ld, norm, lane);
 #pragma unroll
       for (int q = 0; q < Q; ++q) { em[q] *= norm; ein[q] *= norm; }
-      xn = __shfl_sync(0xffffffffu, xn, 0) * norm; xc = __shfl_sync(0xffffffffu, xc, 0) * norm; xj = __shfl_sync(0xffffffffu, xj, 0) * norm;
-      const float xfactor = xn + xc + xj;
       for (int x = 0; x < K; ++x) {
         const float *rp = bm.rfb + (size_t)x * QW;
         float part = 0.0f;
@@ -161,24 +171,7 @@ __global__ void __launch_bounds__(BLK_WARPS * 32) envelope2_kernel(DomdefParams 
         part = warp_sum_float(part);
         if (lane == 0) null2[x] = part + xfactor;
       }
-      __syncwarp();
-      if (lane == 0) {
-        { float r = 0.f; r += null2[2]; r += null2[11]; null2[21] = __fdiv_rn(r, 2.0f); }
-        { float r = 0.f; r += null2[7]; r += null2[9];  null2[22] = __fdiv_rn(r, 2.0f); }
-        { float r = 0.f; r += null2[3]; r += null2[13]; null2[23] = __fdiv_rn(r, 2.0f); }
-        null2[24] = null2[8]; null2[25] = null2[1];
-        float rx = 0.f;
-        for (int x = 0; x < K; ++x) rx += null2[x];
-        null2[26] = __fdiv_rn(rx, 20.0f);
-        null2[20] = 1.0f; null2[27] = 1.0f; null2[28] = 1.0f; null2[29] = 1.0f;
-      }
-      __syncwarp();
-      // per-residue log ratios: 30 table entries, logarithm in double and rounded once (the float value does not depend on
-      // the libm at hand, so the oracle's host arithmetic reproduces it)
-      if (lane < KPAD) null2[lane] = (float)log((double)null2[lane]);
-      __syncwarp();
-      for (int pos = env.i + lane; pos <= env.j; pos += 32) n2sc[pos] = null2[res[pos - env.i]];
-      __syncwarp();
+      null2_finish(null2, n2sc, res, env, lane);
     }
     // ---- optimal accuracy fill: OA matrix overwrites F, specials go to xo ----
     float oasc = 0.0f;
@@ -189,8 +182,8 @@ __global__ void __launch_bounds__(BLK_WARPS * 32) envelope2_kernel(DomdefParams 
       for (int q = 0; q < Q; ++q) { oM[q] = NINF; oI[q] = NINF; oD[q] = NINF; }
 #pragma unroll
       for (int z = 0; z < 3 * Q; ++z) Bm[z * 32 + lane] = NINF;
-      float oE = NINF, oN = 0.0f, oJ = NINF, oC = NINF, oB = (sp.nmove > 0.0f) ? 0.0f : NINF;
-      if (lane == 0) { xo[X_E] = oE; xo[X_N] = oN; xo[X_J] = oJ; xo[X_B] = oB; xo[X_C] = oC; }
+      OaSpecials os(sp);
+      os.store(xo, lane);
       for (int r = 1; r <= Ld; ++r) {
         if (r + 2 <= Ld && lane < Q) {
           const float *fn = F + (int64_t)(r + 2) * 3 * QW;
@@ -211,7 +204,7 @@ __global__ void __launch_bounds__(BLK_WARPS * 32) envelope2_kernel(DomdefParams 
           const float4 t0 = bm.T0(q), t1 = bm.T1(q);
           const bool in = (lane * Q + q + 1) <= M;
           const float pm = (q > 0) ? oM[q - 1] : pm_in, pi = (q > 0) ? oI[q - 1] : pi_in, pd = (q > 0) ? oD[q - 1] : pd_in;
-          float sv = (t0.x > 0.0f) ? oB : 0.0f;
+          float sv = (t0.x > 0.0f) ? os.B : 0.0f;
           sv = fmaxf(sv, (t0.y > 0.0f) ? pm : 0.0f);
           sv = fmaxf(sv, (t0.z > 0.0f) ? pi : 0.0f);
           sv = fmaxf(sv, (t0.w > 0.0f) ? pd : 0.0f);
@@ -247,115 +240,17 @@ __global__ void __launch_bounds__(BLK_WARPS * 32) envelope2_kernel(DomdefParams 
         }
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) emax = fmaxf(emax, __shfl_xor_sync(0xffffffffu, emax, o));
-        oE = emax;
-        const float ppn = pps[r * 3 + 0], ppj = pps[r * 3 + 1], ppc = pps[r * 3 + 2];
-        float t1s = (sp.nloop == 0.0f) ? FLT_MIN_F : 1.0f, t2s = (sp.eloop == 0.0f) ? FLT_MIN_F : 1.0f;
-        oJ = fmaxf(t1s * (oJ + ppj), t2s * oE);
-        t2s = (sp.emove == 0.0f) ? FLT_MIN_F : 1.0f;
-        oC = fmaxf(t1s * (oC + ppc), t2s * oE);
-        oN = t1s * (oN + ppn);
-        t1s = (sp.nmove == 0.0f) ? FLT_MIN_F : 1.0f;
-        oB = fmaxf(t1s * oN, t1s * oJ);
+        os.row(sp, pps + r * 3, emax);
 #pragma unroll
         for (int q = 0; q < Q; ++q) { orow[q * 32] = oM[q]; orow[(Q + q) * 32] = oD[q]; orow[(2 * Q + q) * 32] = oI[q]; }
-        if (lane == 0) { float *xr = xo + (int64_t)r * X_NX; xr[X_E] = oE; xr[X_N] = oN; xr[X_J] = oJ; xr[X_B] = oB; xr[X_C] = oC; }
+        os.store(xo + (int64_t)r * X_NX, lane);
       }
-      oasc = oC;
+      oasc = os.C;
     }
     __syncwarp();
-    // ---- OA traceback (warp-uniform walk; cell (k) lives at q = (k-1) % Q, lane = (k-1) / Q) ----
-    bool ok = !range_err;
-    int hmmfrom = 0, hmmto = 0, sqfrom = 0, sqto = 0;
-#define CELL(row, st, k) Bm[((int64_t)(row) * 3 + (st)) * QW + (((k) - 1) % Q) * 32 + ((k) - 1) / Q]
-#define TT0(k) (__ldg(p.tfb + ms.blk_off * 64 + ((((k) - 1) % Q) * 32 + ((k) - 1) / Q) * 2))
-#define TT1(k) (__ldg(p.tfb + ms.blk_off * 64 + ((((k) - 1) % Q) * 32 + ((k) - 1) / Q) * 2 + 1))
-    if (ok) {
-      int i = Ld, k = 0, s0 = ST_C, s1 = -1;
-      int firstMi = 0, firstMk = 0, lastMi = 0, lastMk = 0; bool have_last = false;
-      int guard = 0;
-      while (s0 != ST_S && ok) {
-        if (++guard > 4 * (Ld + M) + 16) { ok = false; break; }
-        const float *xc = xo + (int64_t)i * X_NX;
-        if (s0 == ST_M) {
-          const float4 t0 = TT0(k);
-          float path[4];
-          path[0] = (t0.y > 0.0f && k > 1) ? CELL(i - 1, 0, k - 1) : -INFINITY;
-          path[1] = (t0.z > 0.0f && k > 1) ? CELL(i - 1, 2, k - 1) : -INFINITY;
-          path[2] = (t0.w > 0.0f && k > 1) ? CELL(i - 1, 1, k - 1) : -INFINITY;
-          path[3] = (t0.x > 0.0f) ? xo[(int64_t)(i - 1) * X_NX + X_B] : -INFINITY;
-          int best = 0;
-          for (int z = 1; z < 4; ++z) if (path[z] > path[best]) best = z;
-          s1 = (best == 0) ? ST_M : (best == 1) ? ST_I : (best == 2) ? ST_D : ST_B;
-          k--; i--;
-        } else if (s0 == ST_D) {
-          const float4 t1 = TT1(k - 1);
-          const float a = (t1.x > 0.0f) ? CELL(i, 0, k - 1) : -INFINITY, b = (t1.w > 0.0f) ? CELL(i, 1, k - 1) : -INFINITY;
-          s1 = (a >= b) ? ST_M : ST_D; k--;
-        } else if (s0 == ST_I) {
-          const float4 t1 = TT1(k);
-          const float a = (t1.y > 0.0f) ? CELL(i - 1, 0, k) : -INFINITY, b = (t1.z > 0.0f) ? CELL(i - 1, 2, k) : -INFINITY;
-          s1 = (a >= b) ? ST_M : ST_I; i--;
-        } else if (s0 == ST_N) {
-          s1 = (i == 0) ? ST_S : ST_N;
-        } else if (s0 == ST_C) {
-          const float t1s = (sp.nloop == 0.0f) ? FLT_MIN_F : 1.0f, t2s = (sp.emove == 0.0f) ? FLT_MIN_F : 1.0f;
-          const float a = (i > 0) ? t1s * (xo[(int64_t)(i - 1) * X_NX + X_C] + pps[i * 3 + 2]) : -INFINITY, b = t2s * xc[X_E];
-          s1 = (a > b) ? ST_C : ST_E;
-        } else if (s0 == ST_J) {
-          const float t1s = (sp.nloop == 0.0f) ? FLT_MIN_F : 1.0f, t2s = (sp.eloop == 0.0f) ? FLT_MIN_F : 1.0f;
-          const float a = (i > 0) ? t1s * (xo[(int64_t)(i - 1) * X_NX + X_J] + pps[i * 3 + 1]) : -INFINITY, b = t2s * xc[X_E];
-          s1 = (a > b) ? ST_J : ST_E;
-        } else if (s0 == ST_E) {
-          const float *dpc = Bm + (int64_t)i * 3 * QW + lane;
-          float bmv = -INFINITY; int bk = -1, bdk = -1; float bd = -INFINITY;
-#pragma unroll
-          for (int q = 0; q < Q; ++q) {
-            const int kk = lane * Q + q + 1;
-            if (kk <= M) {
-              const float v = dpc[q * 32]; if (v >= bmv) { bmv = v; bk = kk; }
-              const float w = dpc[(Q + q) * 32]; if (w > bd) { bd = w; bdk = kk; }
-            }
-          }
-#pragma unroll
-          for (int o = 16; o > 0; o >>= 1) {
-            const float om = __shfl_xor_sync(0xffffffffu, bmv, o); const int ok2 = __shfl_xor_sync(0xffffffffu, bk, o);
-            if (om > bmv || (om == bmv && ok2 > bk)) { bmv = om; bk = ok2; }
-            const float od = __shfl_xor_sync(0xffffffffu, bd, o); const int odk = __shfl_xor_sync(0xffffffffu, bdk, o);
-            if (od > bd || (od == bd && odk >= 0 && (bdk < 0 || odk < bdk))) { bd = od; bdk = odk; }
-          }
-          if (bd > bmv) { s1 = ST_D; k = bdk; } else { s1 = ST_M; k = bk; }
-          if (k < 1) { ok = false; break; }
-        } else if (s0 == ST_B) {
-          const float t1s = (sp.nmove == 0.0f) ? FLT_MIN_F : 1.0f;
-          s1 = (t1s * xc[X_N] > t1s * xc[X_J]) ? ST_N : ST_J;
-        } else { ok = false; break; }
-        if (s1 == ST_M) {
-          if (!have_last || s0 == ST_E) { lastMi = i; lastMk = k; have_last = true; }
-          firstMi = i; firstMk = k;
-          if (p.trace != nullptr && lane == 0) p.trace[pw.row_off + env.i - 1 + i] = k;
-        } else if (s1 == ST_I) {
-          if (p.trace != nullptr && lane == 0) p.trace[pw.row_off + env.i - 1 + i] = -k;
-        }
-        if ((s1 == ST_N || s1 == ST_J || s1 == ST_C) && s1 == s0) i--;
-        s0 = s1;
-      }
-      if (!have_last) ok = false;
-      hmmfrom = firstMk; hmmto = lastMk; sqfrom = firstMi + env.i - 1; sqto = lastMi + env.i - 1;
-    }
-#undef CELL
-#undef TT0
-#undef TT1
-    if (lane == 0) {
-      DomainOut out;
-      out.pair = env.pair; out.ienv = env.i; out.jenv = env.j;
-      float domcorrection = 0.0f;
-      for (int pos = env.i; pos <= env.j; ++pos) domcorrection += n2sc[pos];
-      out.ok = ok ? 1 : 0;
-      out.envsc = envsc; out.oasc = oasc; out.domcorrection = domcorrection;
-      out.hmmfrom = hmmfrom; out.hmmto = hmmto; out.sqfrom = sqfrom; out.sqto = sqto;
-      out.bitscore = 0.f; out.dombias = 0.f; out.pad = 0.f; out.lnP = 0.0;
-      p.doms[env.slot] = out;
-    }
+    OaTrace tr;
+    if (!range_err) tr = oa_traceback(BlockedLayout<Q>{Bm, p.tfb + ms.blk_off * 64, M}, p, pw, env, sp, xo, pps, Ld, M, lane);
+    write_domain(p, env, n2sc, tr, envsc, oasc, lane);
     __syncwarp();
   }
 }
@@ -363,38 +258,20 @@ __global__ void __launch_bounds__(BLK_WARPS * 32) envelope2_kernel(DomdefParams 
 // ------------------------------------------------------------------------------------------------
 // launchers: one launch per class; every launch walks the whole list and picks its own models
 // ------------------------------------------------------------------------------------------------
-template <int Q, bool TSMEM, class P, class KF>
-static int launch_one(KF kern, const P &p, int grid, size_t extra, cudaStream_t st, const char *what) {
-  const size_t smem = (TSMEM ? BLK_WARPS * blk_tsm_bytes<Q>() : 0) + extra;
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return cuda_fail(e, what);
-  }
-  kern<<<grid, BLK_WARPS * 32, smem, st>>>(p);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? CKM_OK : cuda_fail(e, what);
+template <class P, class KF>
+static int launch_blk(KF kern, const char *name, int Q, bool tsmem, const P &p, int grid, size_t extra, cudaStream_t st) {
+  return launch_kernel(kern, name, grid, BLK_WARPS * 32, (tsmem ? BLK_WARPS * blk_tsm_bytes(Q) : 0) + extra, st, p);
 }
-
-#define CKM_CLASS_SWITCH(KERN, EXTRA, WHAT)                                                              \
-  switch (cls) {                                                                                        \
-    case 0: return launch_one<2, false>(KERN<2, false>, p, grid, EXTRA, st, WHAT);                      \
-    case 1: return launch_one<4, false>(KERN<4, false>, p, grid, EXTRA, st, WHAT);                      \
-    case 2: return launch_one<6, false>(KERN<6, false>, p, grid, EXTRA, st, WHAT);                      \
-    case 3: return launch_one<8, false>(KERN<8, false>, p, grid, EXTRA, st, WHAT);                      \
-    case 4: return launch_one<12, true>(KERN<12, true>, p, grid, EXTRA, st, WHAT);                      \
-    case 5: return launch_one<16, true>(KERN<16, true>, p, grid, EXTRA, st, WHAT);                      \
-    case 6: return launch_one<20, true>(KERN<20, true>, p, grid, EXTRA, st, WHAT);                      \
-    case 7: return launch_one<24, true>(KERN<24, true>, p, grid, EXTRA, st, WHAT);                      \
-    case 8: return launch_one<28, true>(KERN<28, true>, p, grid, EXTRA, st, WHAT);                      \
-    case 9: return launch_one<32, true>(KERN<32, true>, p, grid, EXTRA, st, WHAT);                      \
-  }                                                                                                     \
-  set_error(WHAT ": bad class"); return CKM_EINVAL;
-
-int launch_fwd2(const FilterParams &p, int cls, int grid, cudaStream_t st) { CKM_CLASS_SWITCH(fwd2_kernel, 0, "fwd2_kernel") }
-int launch_regions2(const DomdefParams &p, int cls, int grid, cudaStream_t st) { CKM_CLASS_SWITCH(regions2_kernel, 0, "regions2_kernel") }
+int launch_fwd2(const FilterParams &p, int cls, int grid, cudaStream_t st) {
+  return with_class(cls, [&](auto Q, auto TSMEM) { return launch_blk(fwd2_kernel<Q, TSMEM>, "fwd2_kernel", Q, TSMEM, p, grid, 0, st); });
+}
+int launch_regions2(const DomdefParams &p, int cls, int grid, cudaStream_t st) {
+  return with_class(cls, [&](auto Q, auto TSMEM) { return launch_blk(regions2_kernel<Q, TSMEM>, "regions2_kernel", Q, TSMEM, p, grid, 0, st); });
+}
 int launch_envelopes2(const DomdefParams &p, int cls, int grid, cudaStream_t st) {
-  const size_t extra = BLK_WARPS * 32 * sizeof(float);
-  CKM_CLASS_SWITCH(envelope2_kernel, extra, "envelope2_kernel")
+  return with_class(cls, [&](auto Q, auto TSMEM) {
+    return launch_blk(envelope2_kernel<Q, TSMEM>, "envelope2_kernel", Q, TSMEM, p, grid, BLK_WARPS * 32 * sizeof(float), st);
+  });
 }
 
 }  // namespace ckm

@@ -48,6 +48,18 @@ __global__ void __launch_bounds__(FWD_WARPS * 32) regions_kernel(DomdefParams p)
 // ------------------------------------------------------------------------------------------------
 // 5b: rescore one envelope
 // ------------------------------------------------------------------------------------------------
+// the traceback's view of the OA matrix: planes of Mpad cells, position k at column k
+struct ChunkedLayout {
+  const float *F; const float4 *tfv; int M, Mpad;
+  __device__ __forceinline__ float cell(int row, int plane, int k) const { return F[((int64_t)row * 3 + plane) * Mpad + k]; }
+  __device__ __forceinline__ float4 t0(int k) const { return __ldg(tfv + 2 * k); }
+  __device__ __forceinline__ float4 t1(int k) const { return __ldg(tfv + 2 * k + 1); }
+  __device__ __forceinline__ void row_best(int row, int lane, float &bm, int &bk, float &bd, int &bdk) const {
+    const float *dpc = F + (int64_t)row * 3 * Mpad;
+    for (int kk = lane + 1; kk <= M; kk += 32) { const float v = dpc[kk]; if (v >= bm) { bm = v; bk = kk; } }
+    for (int kk = lane + 1; kk <= M; kk += 32) { const float v = dpc[Mpad + kk]; if (v > bd) { bd = v; bdk = kk; } }
+  }
+};
 
 __global__ void __launch_bounds__(FWD_WARPS * 32) envelope_kernel(DomdefParams p) {
   extern __shared__ __align__(16) uint8_t smem[];
@@ -68,11 +80,6 @@ __global__ void __launch_bounds__(FWD_WARPS * 32) envelope_kernel(DomdefParams p
     float *xf = Bm + mat, *xb = xf + (int64_t)(Ld + 1) * X_NX, *pps = xb + (int64_t)(Ld + 1) * X_NX;   // pps: N,J,C posteriors per row
     float *xo = xf;                                                                                   // OA specials reuse xf
     float *n2sc = p.n2sc + pw.row_off;
-    DomainOut out;
-    out.pair = env.pair; out.ienv = env.i; out.jenv = env.j; out.ok = 0;
-    out.hmmfrom = out.hmmto = out.sqfrom = out.sqto = 0; out.envsc = 0.f; out.domcorrection = 0.f; out.oasc = 0.f;
-    out.bitscore = 0.f; out.dombias = 0.f; out.lnP = 0.0;
-
     float envsc;
     forward_rows<true>(fm, res, Ld, sp, rowM, rowI, rowD, lane, xf, F, 0, &envsc);
     __syncwarp();
@@ -90,17 +97,7 @@ __global__ void __launch_bounds__(FWD_WARPS * 32) envelope_kernel(DomdefParams p
         br[2 * Mpad + k] = fr[2 * Mpad + k] * br[2 * Mpad + k] * totr;
       }
     }
-    for (int r = lane; r <= Ld; r += 32) {
-      float pn = 0.f, pj = 0.f, pc = 0.f;
-      if (r >= 1) {
-        const float *f0 = xf + (int64_t)(r - 1) * X_NX, *b1 = xb + (int64_t)r * X_NX;
-        pn = f0[X_N] * b1[X_N] * sp.nloop * scaleproduct;
-        pj = f0[X_J] * b1[X_J] * sp.nloop * scaleproduct;
-        pc = f0[X_C] * b1[X_C] * sp.nloop * scaleproduct;
-      }
-      pps[r * 3 + 0] = pn; pps[r * 3 + 1] = pj; pps[r * 3 + 2] = pc;
-    }
-    __syncwarp();
+    special_posteriors(sp, xf, xb, scaleproduct, pps, Ld, lane);
     const bool range_err = isinf(scaleproduct);
     // ---- null2 by expectation ----
     if (!range_err && !env.null2_done) {
@@ -110,16 +107,9 @@ __global__ void __launch_bounds__(FWD_WARPS * 32) envelope_kernel(DomdefParams p
         for (int r = 2; r <= Ld; ++r) { a += Bm[(int64_t)r * 3 * Mpad + k]; b += Bm[(int64_t)r * 3 * Mpad + 2 * Mpad + k]; }
         em[k] = a; ein[k] = b;
       }
-      float xn = 0.f, xc = 0.f, xj = 0.f;
-      if (lane == 0) {
-        xn = pps[3 + 0]; xj = pps[3 + 1]; xc = pps[3 + 2];
-        for (int r = 2; r <= Ld; ++r) { xn += pps[r * 3 + 0]; xj += pps[r * 3 + 1]; xc += pps[r * 3 + 2]; }
-      }
-      __syncwarp();
       const float norm = __fdiv_rn(1.0f, (float)Ld);
+      const float xfactor = special_xfactor(pps, Ld, norm, lane);
       for (int k = lane + 1; k <= M; k += 32) { em[k] *= norm; ein[k] *= norm; }
-      xn = __shfl_sync(0xffffffffu, xn, 0) * norm; xc = __shfl_sync(0xffffffffu, xc, 0) * norm; xj = __shfl_sync(0xffffffffu, xj, 0) * norm;
-      const float xfactor = xn + xc + xj;
       __syncwarp();
       float *null2 = rowD;     // KP floats
       for (int x = 0; x < K; ++x) {
@@ -129,26 +119,7 @@ __global__ void __launch_bounds__(FWD_WARPS * 32) envelope_kernel(DomdefParams p
         part = warp_sum_float(part);
         if (lane == 0) null2[x] = part + xfactor;
       }
-      __syncwarp();
-      if (lane == 0) {
-        // degenerate residues: plain average of the odds over the set, summed in residue-index order; gap/'*'/'~' = 1
-        { float r = 0.f; r += null2[2]; r += null2[11]; null2[21] = __fdiv_rn(r, 2.0f); }     // B = D|N
-        { float r = 0.f; r += null2[7]; r += null2[9];  null2[22] = __fdiv_rn(r, 2.0f); }     // J = I|L
-        { float r = 0.f; r += null2[3]; r += null2[13]; null2[23] = __fdiv_rn(r, 2.0f); }     // Z = E|Q
-        null2[24] = null2[8];                                                                 // O -> K
-        null2[25] = null2[1];                                                                 // U -> C
-        float rx = 0.f;
-        for (int x = 0; x < K; ++x) rx += null2[x];
-        null2[26] = __fdiv_rn(rx, 20.0f);
-        null2[20] = 1.0f; null2[27] = 1.0f; null2[28] = 1.0f; null2[29] = 1.0f;
-      }
-      __syncwarp();
-      // per-residue log ratios: 30 table entries, logarithm in double and rounded once (the float value does not depend on
-      // the libm at hand, so the oracle's host arithmetic reproduces it)
-      if (lane < KPAD) null2[lane] = (float)log((double)null2[lane]);
-      __syncwarp();
-      for (int pos = env.i + lane; pos <= env.j; pos += 32) n2sc[pos] = null2[res[pos - env.i]];
-      __syncwarp();
+      null2_finish(null2, n2sc, res, env, lane);
     }
     // ---- optimal accuracy fill: OA matrix overwrites the Forward matrix, specials go to xo ----
     float oasc = 0.0f;
@@ -156,8 +127,8 @@ __global__ void __launch_bounds__(FWD_WARPS * 32) envelope_kernel(DomdefParams p
       const float NINF = -INFINITY;
       for (int k = lane; k < 3 * Mpad; k += 32) F[k] = NINF;
       for (int k = lane; k < nchunk * 32 + 1; k += 32) { rowM[k] = NINF; rowI[k] = NINF; rowD[k] = NINF; }
-      float oE = NINF, oN = 0.0f, oJ = NINF, oC = NINF, oB = (sp.nmove > 0.0f) ? 0.0f : NINF;
-      if (lane == 0) { xo[X_E] = oE; xo[X_N] = oN; xo[X_J] = oJ; xo[X_B] = oB; xo[X_C] = oC; }
+      OaSpecials os(sp);
+      os.store(xo, lane);
       __syncwarp();
       for (int r = 1; r <= Ld; ++r) {
         const float *ppr = Bm + (int64_t)r * 3 * Mpad;
@@ -171,7 +142,7 @@ __global__ void __launch_bounds__(FWD_WARPS * 32) envelope_kernel(DomdefParams p
           if (lane == 0) { pm = cM; pi2 = cI; pd = cD; }
           cM = __shfl_sync(0xffffffffu, oM, 31); cI = __shfl_sync(0xffffffffu, oI, 31); cD = __shfl_sync(0xffffffffu, oD, 31);
           const float4 t0 = __ldg(fm.tfv + 2 * k), t1 = __ldg(fm.tfv + 2 * k + 1);
-          float sv = (t0.x > 0.0f) ? oB : 0.0f;
+          float sv = (t0.x > 0.0f) ? os.B : 0.0f;
           sv = fmaxf(sv, (t0.y > 0.0f) ? pm : 0.0f);
           sv = fmaxf(sv, (t0.z > 0.0f) ? pi2 : 0.0f);
           sv = fmaxf(sv, (t0.w > 0.0f) ? pd : 0.0f);
@@ -202,107 +173,16 @@ __global__ void __launch_bounds__(FWD_WARPS * 32) envelope_kernel(DomdefParams p
         (void)dcarry_set;
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) emax = fmaxf(emax, __shfl_xor_sync(0xffffffffu, emax, o));
-        oE = emax;
-        const float ppn = pps[r * 3 + 0], ppj = pps[r * 3 + 1], ppc = pps[r * 3 + 2];
-        float t1s = (sp.nloop == 0.0f) ? FLT_MIN_F : 1.0f, t2s = (sp.eloop == 0.0f) ? FLT_MIN_F : 1.0f;
-        oJ = fmaxf(t1s * (oJ + ppj), t2s * oE);
-        t2s = (sp.emove == 0.0f) ? FLT_MIN_F : 1.0f;
-        oC = fmaxf(t1s * (oC + ppc), t2s * oE);
-        oN = t1s * (oN + ppn);
-        t1s = (sp.nmove == 0.0f) ? FLT_MIN_F : 1.0f;
-        oB = fmaxf(t1s * oN, t1s * oJ);
-        if (lane == 0) { float *xr = xo + (int64_t)r * X_NX; xr[X_E] = oE; xr[X_N] = oN; xr[X_J] = oJ; xr[X_B] = oB; xr[X_C] = oC; }
+        os.row(sp, pps + r * 3, emax);
+        os.store(xo + (int64_t)r * X_NX, lane);
         __syncwarp();
       }
-      oasc = oC;
+      oasc = os.C;
     }
     __syncwarp();
-    // ---- OA traceback: first/last match state of the (single) domain ----
-    bool ok = !range_err;
-    int hmmfrom = 0, hmmto = 0, sqfrom = 0, sqto = 0;
-    if (ok) {
-      int i = Ld, k = 0, s0 = ST_C, s1 = -1;
-      int firstMi = 0, firstMk = 0, lastMi = 0, lastMk = 0; bool have_last = false;
-      int guard = 0;
-      while (s0 != ST_S && ok) {          // warp-uniform state machine; lane 0's reads are broadcast
-        if (++guard > 4 * (Ld + M) + 16) { ok = false; break; }
-        const float *xc = xo + (int64_t)i * X_NX;
-        if (s0 == ST_M) {
-          const float *dpp = F + (int64_t)(i - 1) * 3 * Mpad;
-          const float4 t0 = __ldg(fm.tfv + 2 * k);
-          float path[4];
-          path[0] = (t0.y > 0.0f) ? dpp[k - 1] : -INFINITY;
-          path[1] = (t0.z > 0.0f) ? dpp[2 * Mpad + k - 1] : -INFINITY;
-          path[2] = (t0.w > 0.0f) ? dpp[Mpad + k - 1] : -INFINITY;
-          path[3] = (t0.x > 0.0f) ? xo[(int64_t)(i - 1) * X_NX + X_B] : -INFINITY;
-          int best = 0;
-          for (int z = 1; z < 4; ++z) if (path[z] > path[best]) best = z;
-          s1 = (best == 0) ? ST_M : (best == 1) ? ST_I : (best == 2) ? ST_D : ST_B;
-          k--; i--;
-        } else if (s0 == ST_D) {
-          const float *dpc = F + (int64_t)i * 3 * Mpad;
-          const float4 t1 = __ldg(fm.tfv + 2 * (k - 1) + 1);
-          const float a = (t1.x > 0.0f) ? dpc[k - 1] : -INFINITY, b = (t1.w > 0.0f) ? dpc[Mpad + k - 1] : -INFINITY;
-          s1 = (a >= b) ? ST_M : ST_D; k--;
-        } else if (s0 == ST_I) {
-          const float *dpp = F + (int64_t)(i - 1) * 3 * Mpad;
-          const float4 t1 = __ldg(fm.tfv + 2 * k + 1);
-          const float a = (t1.y > 0.0f) ? dpp[k] : -INFINITY, b = (t1.z > 0.0f) ? dpp[2 * Mpad + k] : -INFINITY;
-          s1 = (a >= b) ? ST_M : ST_I; i--;
-        } else if (s0 == ST_N) {
-          s1 = (i == 0) ? ST_S : ST_N;
-        } else if (s0 == ST_C) {
-          const float t1s = (sp.nloop == 0.0f) ? FLT_MIN_F : 1.0f, t2s = (sp.emove == 0.0f) ? FLT_MIN_F : 1.0f;
-          const float a = (i > 0) ? t1s * (xo[(int64_t)(i - 1) * X_NX + X_C] + pps[i * 3 + 2]) : -INFINITY, b = t2s * xc[X_E];
-          s1 = (a > b) ? ST_C : ST_E;
-        } else if (s0 == ST_J) {
-          const float t1s = (sp.nloop == 0.0f) ? FLT_MIN_F : 1.0f, t2s = (sp.eloop == 0.0f) ? FLT_MIN_F : 1.0f;
-          const float a = (i > 0) ? t1s * (xo[(int64_t)(i - 1) * X_NX + X_J] + pps[i * 3 + 1]) : -INFINITY, b = t2s * xc[X_E];
-          s1 = (a > b) ? ST_J : ST_E;
-        } else if (s0 == ST_E) {
-          // argmax over k of M(i,k) (last maximal index wins ties); a D can only win if strictly greater than every M
-          const float *dpc = F + (int64_t)i * 3 * Mpad;
-          float bm = -INFINITY; int bk = -1;
-          for (int kk = lane + 1; kk <= M; kk += 32) { const float v = dpc[kk]; if (v >= bm) { bm = v; bk = kk; } }
-#pragma unroll
-          for (int o = 16; o > 0; o >>= 1) {
-            const float om = __shfl_xor_sync(0xffffffffu, bm, o); const int ok2 = __shfl_xor_sync(0xffffffffu, bk, o);
-            if (om > bm || (om == bm && ok2 > bk)) { bm = om; bk = ok2; }
-          }
-          float bd = -INFINITY; int bdk = -1;
-          for (int kk = lane + 1; kk <= M; kk += 32) { const float v = dpc[Mpad + kk]; if (v > bd) { bd = v; bdk = kk; } }
-#pragma unroll
-          for (int o = 16; o > 0; o >>= 1) {
-            const float om = __shfl_xor_sync(0xffffffffu, bd, o); const int ok2 = __shfl_xor_sync(0xffffffffu, bdk, o);
-            if (om > bd || (om == bd && ok2 >= 0 && (bdk < 0 || ok2 < bdk))) { bd = om; bdk = ok2; }
-          }
-          if (bd > bm) { s1 = ST_D; k = bdk; } else { s1 = ST_M; k = bk; }
-          if (k < 1) { ok = false; break; }
-        } else if (s0 == ST_B) {
-          const float t1s = (sp.nmove == 0.0f) ? FLT_MIN_F : 1.0f;
-          s1 = (t1s * xc[X_N] > t1s * xc[X_J]) ? ST_N : ST_J;
-        } else { ok = false; break; }
-        if (s1 == ST_M) {
-          if (!have_last || s0 == ST_E) { lastMi = i; lastMk = k; have_last = true; }
-          firstMi = i; firstMk = k;
-          if (p.trace != nullptr && lane == 0) p.trace[pw.row_off + env.i - 1 + i] = k;
-        } else if (s1 == ST_I) {
-          if (p.trace != nullptr && lane == 0) p.trace[pw.row_off + env.i - 1 + i] = -k;
-        }
-        if ((s1 == ST_N || s1 == ST_J || s1 == ST_C) && s1 == s0) i--;
-        s0 = s1;
-      }
-      if (!have_last) ok = false;
-      hmmfrom = firstMk; hmmto = lastMk; sqfrom = firstMi + env.i - 1; sqto = lastMi + env.i - 1;
-    }
-    if (lane == 0) {
-      float domcorrection = 0.0f;
-      for (int pos = env.i; pos <= env.j; ++pos) domcorrection += n2sc[pos];
-      out.ok = ok ? 1 : 0;
-      out.envsc = envsc; out.oasc = oasc; out.domcorrection = domcorrection;
-      out.hmmfrom = hmmfrom; out.hmmto = hmmto; out.sqfrom = sqfrom; out.sqto = sqto;
-      p.doms[env.slot] = out;
-    }
+    OaTrace tr;
+    if (!range_err) tr = oa_traceback(ChunkedLayout{F, fm.tfv, M, Mpad}, p, pw, env, sp, xo, pps, Ld, M, lane);
+    write_domain(p, env, n2sc, tr, envsc, oasc, lane);
     __syncwarp();
   }
 }
@@ -366,25 +246,11 @@ __global__ void __launch_bounds__(128) scores_kernel(DomdefParams p) {
 }
 
 int launch_regions(const DomdefParams &p, int grid, cudaStream_t st) {
-  const size_t smem = (size_t)FWD_WARPS * 3 * p.row_elems * sizeof(float);
-  cudaError_t e = cudaFuncSetAttribute(regions_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(regions)");
-  regions_kernel<<<grid, FWD_WARPS * 32, smem, st>>>(p);
-  e = cudaGetLastError();
-  return e == cudaSuccess ? CKM_OK : cuda_fail(e, "regions_kernel launch");
+  return launch_kernel(regions_kernel, "regions_kernel", grid, FWD_WARPS * 32, (size_t)FWD_WARPS * 3 * p.row_elems * sizeof(float), st, p);
 }
 int launch_envelopes(const DomdefParams &p, int grid, cudaStream_t st) {
-  const size_t smem = (size_t)FWD_WARPS * 3 * p.row_elems * sizeof(float);
-  cudaError_t e = cudaFuncSetAttribute(envelope_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(envelope)");
-  envelope_kernel<<<grid, FWD_WARPS * 32, smem, st>>>(p);
-  e = cudaGetLastError();
-  return e == cudaSuccess ? CKM_OK : cuda_fail(e, "envelope_kernel launch");
+  return launch_kernel(envelope_kernel, "envelope_kernel", grid, FWD_WARPS * 32, (size_t)FWD_WARPS * 3 * p.row_elems * sizeof(float), st, p);
 }
-int launch_scores(const DomdefParams &p, int grid, cudaStream_t st) {
-  scores_kernel<<<grid, 128, 0, st>>>(p);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? CKM_OK : cuda_fail(e, "scores_kernel launch");
-}
+int launch_scores(const DomdefParams &p, int grid, cudaStream_t st) { return launch_kernel(scores_kernel, "scores_kernel", grid, 128, 0, st, p); }
 
 }  // namespace ckm

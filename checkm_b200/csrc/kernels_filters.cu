@@ -9,6 +9,7 @@
 #include "device_utils.cuh"
 #include "stages.hpp"
 #include "fwdback.cuh"
+#include "filter_common.cuh"
 
 namespace ckm {
 
@@ -55,9 +56,7 @@ __global__ void __launch_bounds__(128) bias_kernel(FilterParams p) {
     if (p.dense_filtersc != nullptr) p.dense_filtersc[(int64_t)p.model_slot[m] * p.nseq + s] = filtersc;
     if (P <= p.F1) {
       cd.filtersc = filtersc; cd.P = P;
-      const int pos = atomicAdd(p.out_count, 1);
-      if (pos < p.out_cap) p.out[pos] = cd;
-      if (p.dense_passed != nullptr) atomicOr_u8(p.dense_passed, (int64_t)p.model_slot[m] * p.nseq + s, 2);
+      filter_pass(p, cd, 2);
     }
   }
 }
@@ -134,25 +133,9 @@ __global__ void __launch_bounds__(VIT_WARPS * 32) vit_kernel(FilterParams p) {
         xC = max(xC, -32768); xJ = max(xJ, -32768); xB = max(xB, -32768);
         __syncwarp();
       }
-      float vsc;
-      if (overflow) vsc = INFINITY;
-      else if (xC > -32768) {
-        vsc = __fsub_rn(__fadd_rn((float)xC, (float)tmove), (float)ms.base_w);
-        vsc = __fdiv_rn(vsc, ms.scale_w);
-        vsc = __fsub_rn(vsc, 3.0f);
-      } else vsc = -INFINITY;
-      cd.vitsc = vsc;
-      const float seq_score = __fdiv_rn(__fsub_rn(vsc, cd.filtersc), 0.69314718055994529f);
-      const double P = gumbel_surv((double)seq_score, (double)ms.evparam[2], (double)ms.evparam[3]);
-      cd.P = P;
-      pass = (P <= p.F2);
-      if (lane == 0 && p.dense_vit != nullptr) p.dense_vit[(int64_t)p.model_slot[m] * p.nseq + s] = vsc;
+      pass = vit_verdict(p, cd, vit_score(overflow, xC, tmove, ms), ms, lane);
     }
-    if (lane == 0 && pass) {
-      const int pos = atomicAdd(p.out_count, 1);
-      if (pos < p.out_cap) p.out[pos] = cd;
-      if (p.dense_passed != nullptr) atomicOr_u8(p.dense_passed, (int64_t)p.model_slot[m] * p.nseq + s, 4);
-    }
+    if (lane == 0 && pass) filter_pass(p, cd, 4);
     __syncwarp();
   }
 }
@@ -270,25 +253,9 @@ __global__ void __launch_bounds__(128) vit2_kernel(FilterParams p) {
           }
         }
       }
-      float vsc;
-      if (overflow) vsc = INFINITY;
-      else if (xC > -32768) {
-        vsc = __fsub_rn(__fadd_rn((float)xC, (float)tmove), (float)ms.base_w);
-        vsc = __fdiv_rn(vsc, ms.scale_w);
-        vsc = __fsub_rn(vsc, 3.0f);
-      } else vsc = -INFINITY;
-      cd.vitsc = vsc;
-      const float seq_score = __fdiv_rn(__fsub_rn(vsc, cd.filtersc), 0.69314718055994529f);
-      const double P = gumbel_surv((double)seq_score, (double)ms.evparam[2], (double)ms.evparam[3]);
-      cd.P = P;
-      pass = (P <= p.F2);
-      if (lane == 0 && p.dense_vit != nullptr) p.dense_vit[(int64_t)p.model_slot[m] * p.nseq + s] = vsc;
+      pass = vit_verdict(p, cd, vit_score(overflow, xC, tmove, ms), ms, lane);
     }
-    if (lane == 0 && pass) {
-      const int pos = atomicAdd(p.out_count, 1);
-      if (pos < p.out_cap) p.out[pos] = cd;
-      if (p.dense_passed != nullptr) atomicOr_u8(p.dense_passed, (int64_t)p.model_slot[m] * p.nseq + s, 4);
-    }
+    if (lane == 0 && pass) filter_pass(p, cd, 4);
 #undef TRQ
   }
 }
@@ -315,68 +282,22 @@ __global__ void __launch_bounds__(FWD_WARPS * 32) fwd_kernel(FilterParams p) {
     const Specials sp = make_specials(L, true);
     float fsc;
     forward_rows<false>(fm, res, L, sp, rowM, rowI, rowD, lane, nullptr, nullptr, 0, &fsc);
-    cd.fwdsc = fsc;
-    const float seq_score = __fdiv_rn(__fsub_rn(fsc, cd.filtersc), 0.69314718055994529f);
-    const double P = exp_surv((double)seq_score, (double)ms.evparam[4], (double)ms.evparam[5]);
-    cd.P = P;
-    if (lane == 0) {
-      if (p.dense_fwd != nullptr) p.dense_fwd[(int64_t)p.model_slot[m] * p.nseq + s] = fsc;
-      if (P <= p.F3) {
-        const int pos = atomicAdd(p.out_count, 1);
-        if (pos < p.out_cap) p.out[pos] = cd;
-        if (p.dense_passed != nullptr) atomicOr_u8(p.dense_passed, (int64_t)p.model_slot[m] * p.nseq + s, 8);
-      }
-    }
+    fwd_verdict(p, cd, fsc, ms, lane);
     __syncwarp();
   }
 }
 
-int launch_bias(const FilterParams &p, int grid, cudaStream_t st) {
-  bias_kernel<<<grid, 128, 0, st>>>(p);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? CKM_OK : cuda_fail(e, "bias_kernel launch");
-}
-template <int Q, bool TSMEM>
-static int launch_vit2_q(const FilterParams &p, int grid, cudaStream_t st) {
-  const int sm = TSMEM ? 4 * Q * 32 * (int)sizeof(uint4) : 0;
-  if (sm > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(vit2_kernel<Q, TSMEM>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm);
-    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(vit2)");
-  }
-  vit2_kernel<Q, TSMEM><<<grid, 128, sm, st>>>(p);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? CKM_OK : cuda_fail(e, "vit2_kernel launch");
-}
+int launch_bias(const FilterParams &p, int grid, cudaStream_t st) { return launch_kernel(bias_kernel, "bias_kernel", grid, 128, 0, st, p); }
 int launch_vit2(const FilterParams &p, int cls, int grid, cudaStream_t st) {
-  switch (cls) {
-    case 0: return launch_vit2_q<2, false>(p, grid, st);
-    case 1: return launch_vit2_q<4, false>(p, grid, st);
-    case 2: return launch_vit2_q<6, false>(p, grid, st);
-    case 3: return launch_vit2_q<8, false>(p, grid, st);
-    case 4: return launch_vit2_q<12, true>(p, grid, st);
-    case 5: return launch_vit2_q<16, true>(p, grid, st);
-    case 6: return launch_vit2_q<20, true>(p, grid, st);
-    case 7: return launch_vit2_q<24, true>(p, grid, st);
-    case 8: return launch_vit2_q<28, true>(p, grid, st);
-    case 9: return launch_vit2_q<32, true>(p, grid, st);
-  }
-  set_error("launch_vit2: bad class"); return CKM_EINVAL;
+  return with_class(cls, [&](auto Q, auto TSMEM) {
+    return launch_kernel(vit2_kernel<Q, TSMEM>, "vit2_kernel", grid, 128, TSMEM ? 4 * Q * 32 * sizeof(uint4) : 0, st, p);
+  });
 }
 int launch_vit(const FilterParams &p, int grid, cudaStream_t st) {
-  const size_t smem = (size_t)VIT_WARPS * 3 * p.row_elems * sizeof(int16_t);
-  cudaError_t e = cudaFuncSetAttribute(vit_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(vit)");
-  vit_kernel<<<grid, VIT_WARPS * 32, smem, st>>>(p);
-  e = cudaGetLastError();
-  return e == cudaSuccess ? CKM_OK : cuda_fail(e, "vit_kernel launch");
+  return launch_kernel(vit_kernel, "vit_kernel", grid, VIT_WARPS * 32, (size_t)VIT_WARPS * 3 * p.row_elems * sizeof(int16_t), st, p);
 }
 int launch_fwd(const FilterParams &p, int grid, cudaStream_t st) {
-  const size_t smem = (size_t)FWD_WARPS * 3 * p.row_elems * sizeof(float);
-  cudaError_t e = cudaFuncSetAttribute(fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(fwd)");
-  fwd_kernel<<<grid, FWD_WARPS * 32, smem, st>>>(p);
-  e = cudaGetLastError();
-  return e == cudaSuccess ? CKM_OK : cuda_fail(e, "fwd_kernel launch");
+  return launch_kernel(fwd_kernel, "fwd_kernel", grid, FWD_WARPS * 32, (size_t)FWD_WARPS * 3 * p.row_elems * sizeof(float), st, p);
 }
 
 }  // namespace ckm

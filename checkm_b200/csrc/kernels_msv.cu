@@ -16,6 +16,7 @@
 #include "engine.hpp"
 #include "device_utils.cuh"
 #include "stages.hpp"
+#include "filter_common.cuh"
 
 namespace ckm {
 
@@ -191,22 +192,8 @@ __global__ void __launch_bounds__(SSV_WARPS * 32, 1) ssv_kernel(SsvParams p) {
               const int tjbm = min(tjb + (int)ms.tbm_b, 255);
               const int xB0 = max((int)ms.base_b - tjbm, 0);
               const int xJ = max(umax + xB0 - (int)ms.tec_b, 0);
-              float usc = ((float)(xJ - tjb) - (float)ms.base_b);
-              usc = __fdiv_rn(usc, ms.scale_b);
-              usc = __fsub_rn(usc, 3.0f);
-              if (p.xj_dense != nullptr) p.xj_dense[(int64_t)p.model_slot[tm.model] * p.nseq + s] = xJ;
-              const float nullsc = p.nullsc[s];
-              const float seq_score = __fdiv_rn(__fsub_rn(usc, nullsc), 0.69314718055994529f);
-              const double P = gumbel_surv((double)seq_score, (double)ms.evparam[0], (double)ms.evparam[1]);
               atomicAdd(p.resolved_count, 1);
-              if (P <= p.F1) {
-                const int pos = atomicAdd(p.pass_count, 1);
-                if (pos < p.pass_cap) {
-                  Candidate cd;
-                  cd.seq = s; cd.model = tm.model; cd.usc = usc; cd.filtersc = nullsc; cd.vitsc = 0.f; cd.fwdsc = 0.f; cd.P = P;
-                  p.pass[pos] = cd;
-                }
-              }
+              msv_out(p, p.pass, p.pass_count, p.pass_cap, s, tm.model, ms, msv_usc(false, xJ, tjb, ms), xJ);
             }
           }
         }
@@ -234,33 +221,14 @@ template __global__ void ssv_kernel<16>(SsvParams);
 template __global__ void ssv_kernel<32>(SsvParams);
 
 int launch_ssv(int J, const SsvParams &p, int grid, size_t smem_bytes, cudaStream_t stream) {
-  cudaError_t e;
+  const int block = SSV_WARPS * 32;
   switch (J) {
-    case 4:
-      e = cudaFuncSetAttribute(ssv_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
-      if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(ssv<4>)");
-      ssv_kernel<4><<<grid, SSV_WARPS * 32, smem_bytes, stream>>>(p);
-      break;
-    case 8:
-      e = cudaFuncSetAttribute(ssv_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
-      if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(ssv<8>)");
-      ssv_kernel<8><<<grid, SSV_WARPS * 32, smem_bytes, stream>>>(p);
-      break;
-    case 16:
-      e = cudaFuncSetAttribute(ssv_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
-      if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(ssv<16>)");
-      ssv_kernel<16><<<grid, SSV_WARPS * 32, smem_bytes, stream>>>(p);
-      break;
-    case 32:
-      e = cudaFuncSetAttribute(ssv_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
-      if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(ssv<32>)");
-      ssv_kernel<32><<<grid, SSV_WARPS * 32, smem_bytes, stream>>>(p);
-      break;
-    default: set_error("unsupported tile width"); return CKM_EINVAL;
+    case 4: return launch_kernel(ssv_kernel<4>, "ssv_kernel<4>", grid, block, smem_bytes, stream, p);
+    case 8: return launch_kernel(ssv_kernel<8>, "ssv_kernel<8>", grid, block, smem_bytes, stream, p);
+    case 16: return launch_kernel(ssv_kernel<16>, "ssv_kernel<16>", grid, block, smem_bytes, stream, p);
+    case 32: return launch_kernel(ssv_kernel<32>, "ssv_kernel<32>", grid, block, smem_bytes, stream, p);
   }
-  e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "ssv_kernel launch");
-  return CKM_OK;
+  set_error("unsupported tile width"); return CKM_EINVAL;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -310,27 +278,7 @@ __global__ void __launch_bounds__(MSV_WARPS * 32) msv_exact_kernel(MsvParams p) 
       uint8_t *tmp = prev; prev = cur; cur = tmp;
     }
     __syncwarp();
-    if (lane == 0) {
-      float usc;
-      if (overflow) usc = INFINITY;
-      else {
-        usc = ((float)(xJ - tjb) - (float)base);
-        usc = __fdiv_rn(usc, ms.scale_b);
-        usc = __fsub_rn(usc, 3.0f);
-      }
-      if (p.xj_dense != nullptr) p.xj_dense[(int64_t)p.model_slot[m] * p.nseq + s] = overflow ? 256 : xJ;
-      const float nullsc = p.nullsc[s];
-      const float seq_score = __fdiv_rn(__fsub_rn(usc, nullsc), 0.69314718055994529f);
-      const double P = gumbel_surv((double)seq_score, (double)ms.evparam[0], (double)ms.evparam[1]);
-      if (P <= p.F1) {
-        const int pos = atomicAdd(p.out_count, 1);
-        if (pos < p.out_cap) {
-          Candidate cd;
-          cd.seq = s; cd.model = m; cd.usc = usc; cd.filtersc = nullsc; cd.vitsc = 0.f; cd.fwdsc = 0.f; cd.P = P;
-          p.out[pos] = cd;
-        }
-      }
-    }
+    if (lane == 0) msv_out(p, p.out, p.out_count, p.out_cap, s, m, ms, msv_usc(overflow, xJ, tjb, ms), overflow ? 256 : xJ);
   }
 }
 
@@ -475,46 +423,12 @@ __global__ void __launch_bounds__(128) msv2_kernel(MsvParams p) {
         else { xe = max(xe - tec, 0); xJ = max(xJ, xe); xB = max(max(base, xJ) - tjbm, 0); }
       }
     }
-    if (lane == 0) {
-      float usc;
-      if (overflow) usc = INFINITY;
-      else {
-        usc = ((float)(xJ - tjb) - (float)base);
-        usc = __fdiv_rn(usc, ms.scale_b);
-        usc = __fsub_rn(usc, 3.0f);
-      }
-      if (p.xj_dense != nullptr) p.xj_dense[(int64_t)p.model_slot[m] * p.nseq + s] = overflow ? 256 : xJ;
-      const float nullsc = p.nullsc[s];
-      const float seq_score = __fdiv_rn(__fsub_rn(usc, nullsc), 0.69314718055994529f);
-      const double P = gumbel_surv((double)seq_score, (double)ms.evparam[0], (double)ms.evparam[1]);
-      if (P <= p.F1) {
-        const int pos = atomicAdd(p.out_count, 1);
-        if (pos < p.out_cap) {
-          Candidate cd;
-          cd.seq = s; cd.model = m; cd.usc = usc; cd.filtersc = nullsc; cd.vitsc = 0.f; cd.fwdsc = 0.f; cd.P = P;
-          p.out[pos] = cd;
-        }
-      }
-    }
+    if (lane == 0) msv_out(p, p.out, p.out_count, p.out_cap, s, m, ms, msv_usc(overflow, xJ, tjb, ms), overflow ? 256 : xJ);
   }
 }
 
 int launch_msv2(const MsvParams &p, int cls, int grid, cudaStream_t stream) {
-  switch (cls) {
-    case 0: msv2_kernel<2><<<grid, 128, 0, stream>>>(p); break;
-    case 1: msv2_kernel<4><<<grid, 128, 0, stream>>>(p); break;
-    case 2: msv2_kernel<6><<<grid, 128, 0, stream>>>(p); break;
-    case 3: msv2_kernel<8><<<grid, 128, 0, stream>>>(p); break;
-    case 4: msv2_kernel<12><<<grid, 128, 0, stream>>>(p); break;
-    case 5: msv2_kernel<16><<<grid, 128, 0, stream>>>(p); break;
-    case 6: msv2_kernel<20><<<grid, 128, 0, stream>>>(p); break;
-    case 7: msv2_kernel<24><<<grid, 128, 0, stream>>>(p); break;
-    case 8: msv2_kernel<28><<<grid, 128, 0, stream>>>(p); break;
-    case 9: msv2_kernel<32><<<grid, 128, 0, stream>>>(p); break;
-    default: set_error("launch_msv2: bad class"); return CKM_EINVAL;
-  }
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? CKM_OK : cuda_fail(e, "msv2_kernel launch");
+  return with_class(cls, [&](auto Q, auto) { return launch_kernel(msv2_kernel<Q>, "msv2_kernel", grid, 128, 0, stream, p); });
 }
 
 // Models too long for a chain of SSV tiles (models.cu: ssv_bypass) skip the pre-filter: all of their pairs become candidates.
@@ -536,19 +450,12 @@ int launch_ssv_bypass(const int32_t *models, int32_t nbypass, int32_t nseq, cons
   if (nbypass <= 0 || nseq <= 0) return CKM_OK;
   const int64_t n = (int64_t)nbypass * nseq;
   const int grid = (int)std::min<int64_t>(1184, (n + 255) / 256);
-  ssv_bypass_kernel<<<grid, 256, 0, stream>>>(models, nbypass, nseq, len, bin, model_active, nmodels_db, cand, cand_count, cand_cap);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? CKM_OK : cuda_fail(e, "ssv_bypass_kernel launch");
+  return launch_kernel(ssv_bypass_kernel, "ssv_bypass_kernel", grid, 256, 0, stream, models, nbypass, nseq, len, bin, model_active,
+                       nmodels_db, cand, cand_count, cand_cap);
 }
 
 int launch_msv_exact(const MsvParams &p, int grid, cudaStream_t stream) {
-  const size_t smem = (size_t)MSV_WARPS * 2 * p.row_bytes;
-  cudaError_t e = cudaFuncSetAttribute(msv_exact_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(msv_exact)");
-  msv_exact_kernel<<<grid, MSV_WARPS * 32, smem, stream>>>(p);
-  e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "msv_exact_kernel launch");
-  return CKM_OK;
+  return launch_kernel(msv_exact_kernel, "msv_exact_kernel", grid, MSV_WARPS * 32, (size_t)MSV_WARPS * 2 * p.row_bytes, stream, p);
 }
 
 }  // namespace ckm

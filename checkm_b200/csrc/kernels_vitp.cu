@@ -24,6 +24,7 @@
 #include "engine.hpp"
 #include "device_utils.cuh"
 #include "stages.hpp"
+#include "filter_common.cuh"
 
 namespace ckm {
 
@@ -33,19 +34,6 @@ constexpr uint32_t VP_TFLOORW = 0xC000C000u;     // -16384 | -16384 : floor of t
 
 __device__ __forceinline__ int vp_lo(uint32_t w) { return (int)(int16_t)(w & 0xffffu); }
 __device__ __forceinline__ int vp_hi(uint32_t w) { return (int)w >> 16; }
-
-// the two ways out of the stage besides the score list: the pass list (P <= F2) and the int32 kernels' redo list
-__device__ __forceinline__ void vit_pass(const FilterParams &p, const Candidate &cd) {
-  const int pos = atomicAdd(p.out_count, 1);
-  if (pos < p.out_cap) p.out[pos] = cd;
-  if (p.dense_passed != nullptr) atomicOr_u8(p.dense_passed, (int64_t)p.model_slot[cd.model] * p.nseq + cd.seq, 4);
-}
-__device__ __forceinline__ void vit_redo(const FilterParams &p, const Candidate &cd) {
-  const int pos = atomicAdd(p.redo_count, 1);
-  if (pos < p.redo_cap) p.redo[pos] = cd;
-}
-// lane-block class (index into BLK_Q) of a model's vq; -1: no class
-__device__ __forceinline__ int vitp_class(int vq) { return vq == 0 ? -1 : (vq <= 8 ? vq / 2 - 1 : vq / 4 + 1); }
 
 // Grouping the survivor list by (class, model), in three passes over p.in.  Count: pairs that need no packed scoring leave
 // here -- P already <= F2 to the pass list, models without a class to the redo list -- and the others are counted per model.
@@ -57,7 +45,7 @@ __global__ void vit_count_kernel(FilterParams p, int32_t *cnt) {
   const int n = min(*p.in_count, p.in_cap);
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const Candidate cd = p.in[i];
-    if (!(cd.P > p.F2)) vit_pass(p, cd);
+    if (!(cd.P > p.F2)) filter_pass(p, cd, 4);
     else if (p.ms[cd.model].vq == 0) vit_redo(p, cd);
     else atomicAdd(cnt + cd.model, 1);
   }
@@ -71,7 +59,7 @@ __global__ void __launch_bounds__(1024) vit_scan_kernel(FilterParams p, int32_t 
     if (threadIdx.x == 0) p.vit_cls_chunks[c] = run_chunks;
     for (int b = 0; b < nmodels; b += 1024) {
       const int m = b + threadIdx.x;
-      const int v = (m < nmodels && vitp_class(p.ms[m].vq) == c) ? cnt[m] : 0, h = (v + VITP_CHUNK - 1) / VITP_CHUNK;
+      const int v = (m < nmodels && blk_class(p.ms[m].vq) == c) ? cnt[m] : 0, h = (v + VITP_CHUNK - 1) / VITP_CHUNK;
       int sv = v, sh = h;
 #pragma unroll
       for (int o = 1; o < 32; o <<= 1) {
@@ -272,41 +260,18 @@ __global__ void __launch_bounds__(VITP_THREADS, vitp_min_blocks(W)) vitp_kernel(
           wcur = wnext;
         }
         if (!redo && xC <= VP_FLOOR + e_move) redo = true;      // a floored row may have set xC (or nothing scored at all)
-        if (!redo) {
-          vsc = __fsub_rn(__fadd_rn((float)xC, (float)tmove), (float)ms.base_w);
-          vsc = __fdiv_rn(vsc, ms.scale_w);
-          vsc = __fsub_rn(vsc, 3.0f);
-        }
+        if (!redo) vsc = vit_vsc(xC, tmove, ms);
       }
       Candidate cd = *cin;
       if (redo) {
         if (lane == 0) vit_redo(p, cd);
         continue;
       }
-      cd.vitsc = vsc;
-      const float seq_score = __fdiv_rn(__fsub_rn(vsc, cd.filtersc), 0.69314718055994529f);
-      const double P = gumbel_surv((double)seq_score, (double)ms.evparam[2], (double)ms.evparam[3]);
-      cd.P = P;
-      if (lane == 0) {
-        if (p.dense_vit != nullptr) p.dense_vit[(int64_t)p.model_slot[cd.model] * p.nseq + s] = vsc;
-        if (P <= p.F2) vit_pass(p, cd);
-      }
+      if (vit_verdict(p, cd, vsc, ms, lane) && lane == 0) filter_pass(p, cd, 4);
     }   // pairs of this chunk
 #undef TR0
 #undef TR1
   }   // chunks
-}
-
-template <int W, bool TSMEM>
-static int launch_vitp_w(const FilterParams &p, int cls, int grid, cudaStream_t st) {
-  constexpr int sm = vitp_smem_bytes(W, TSMEM);
-  if (sm > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(vitp_kernel<W, TSMEM>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm);
-    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(vitp)");
-  }
-  vitp_kernel<W, TSMEM><<<grid, VITP_THREADS, sm, st>>>(p, cls);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? CKM_OK : cuda_fail(e, "vitp_kernel launch");
 }
 
 // every (model slot, sequence) pair as a candidate that still needs the Viterbi filter (parity entry point ckm_viterbi_scores)
@@ -320,25 +285,13 @@ __global__ void all_pairs_kernel(Candidate *out, int32_t *count, const int32_t *
   if (blockIdx.x == 0 && threadIdx.x == 0) *count = (int32_t)n;
 }
 int launch_all_pairs(Candidate *out, int32_t *count, const int32_t *slot_model, int32_t nslots, int32_t nseq, cudaStream_t st) {
-  all_pairs_kernel<<<592, 256, 0, st>>>(out, count, slot_model, nslots, nseq);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? CKM_OK : cuda_fail(e, "all_pairs_kernel launch");
+  return launch_kernel(all_pairs_kernel, "all_pairs_kernel", 592, 256, 0, st, out, count, slot_model, nslots, nseq);
 }
 
 int launch_vitp(const FilterParams &p, int cls, int grid, cudaStream_t st) {
-  switch (cls) {
-    case 0: return launch_vitp_w<1, false>(p, cls, grid, st);
-    case 1: return launch_vitp_w<2, false>(p, cls, grid, st);
-    case 2: return launch_vitp_w<3, false>(p, cls, grid, st);
-    case 3: return launch_vitp_w<4, false>(p, cls, grid, st);
-    case 4: return launch_vitp_w<6, true>(p, cls, grid, st);
-    case 5: return launch_vitp_w<8, true>(p, cls, grid, st);
-    case 6: return launch_vitp_w<10, true>(p, cls, grid, st);
-    case 7: return launch_vitp_w<12, true>(p, cls, grid, st);
-    case 8: return launch_vitp_w<14, true>(p, cls, grid, st);
-    case 9: return launch_vitp_w<16, true>(p, cls, grid, st);
-  }
-  set_error("launch_vitp: bad class"); return CKM_EINVAL;
+  return with_class(cls, [&](auto Q, auto TSMEM) {
+    return launch_kernel(vitp_kernel<Q / 2, TSMEM>, "vitp_kernel", grid, VITP_THREADS, vitp_smem_bytes(Q / 2, TSMEM), st, p, cls);
+  });
 }
 
 }  // namespace ckm

@@ -6,6 +6,7 @@
 #include <fstream>
 #include <stdexcept>
 #include "engine.hpp"
+#include "stages.hpp"
 
 namespace ckm {
 
@@ -190,7 +191,7 @@ int models_build_device(ckm_models &db) {
       for (int k = 1; k <= m.M; ++k) tbm = std::min(tbm, (int)m.twv[(size_t)k * T_N + 0]);
       s.vit_emax = (int16_t)emax; s.vit_tbm = (int16_t)tbm;
     }
-    s.vq = (m.M <= 64) ? 2 : (m.M <= 128) ? 4 : (m.M <= 192) ? 6 : (m.M <= 256) ? 8 : (m.M <= 384) ? 12 : (m.M <= 512) ? 16 : (m.M <= 640) ? 20 : (m.M <= 768) ? 24 : (m.M <= 896) ? 28 : (m.M <= 1024) ? 32 : 0;
+    s.vq = vq_of(m.M);
     s.blk_off = blk_units;
     s.msv2_ok = (s.vq != 0 && (int)m.base_b + (int)m.bias_b < 255) ? 1 : 0;
     blk_units += s.vq;

@@ -78,13 +78,7 @@ struct Trace {
   }
 };
 
-static int vq_of(int M) { return (M <= 64) ? 2 : (M <= 128) ? 4 : (M <= 192) ? 6 : (M <= 256) ? 8 : (M <= 384) ? 12 : (M <= 512) ? 16 : (M <= 640) ? 20 : (M <= 768) ? 24 : (M <= 896) ? 28 : (M <= 1024) ? 32 : 0; }
-static int cls_of(int M, bool use_blk) {      // class index: 0..9 lane-block classes, 10 = unblocked kernels
-  if (!use_blk) return N_BLK_CLASSES;
-  const int q = vq_of(M);
-  for (int c = 0; c < N_BLK_CLASSES; ++c) if (BLK_Q[c] == q) return c;
-  return N_BLK_CLASSES;
-}
+static int cls_of(int M, bool use_blk) { return use_blk ? blk_class(vq_of(M)) : N_BLK_CLASSES; }
 
 // the per-class launches of one stage go to the engine's class streams: fork after the main stream, join back into it
 static int fan_out(ckm_engine *e) {

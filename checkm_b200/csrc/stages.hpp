@@ -1,5 +1,6 @@
 // stages.hpp -- parameter blocks and launchers of the device stages (kernels_*.cu), shared with search.cu.
 #pragma once
+#include <type_traits>
 #include "engine.hpp"
 
 namespace ckm {
@@ -51,7 +52,7 @@ struct MsvParams {
   const int32_t *model_slot;   // database model index -> row of xj_dense
   int32_t nseq;
   int32_t row_bytes;           // shared-memory bytes of one DP row (>= maxM+2)
-  int32_t use_blk;             // 1: models with msv2_ok go to the lane-blocked kernels, 0: every candidate to msv_exact_kernel
+  int32_t use_blk;             // 1: models with msv2_ok go to msv2_kernel<Q>, 0 (CKM_BLK=0): every candidate to msv_exact_kernel
   double F1;
 };
 
@@ -81,16 +82,51 @@ struct FilterParams {
   Candidate *out; int32_t *out_count; int32_t out_cap;
   int32_t row_elems;                 // shared-memory elements of one DP row
   double F1, F2, F3;
-  int32_t use_blk;                   // 1: models with a blocked class go to the *2 kernels
+  int32_t use_blk;                   // 1: models with a class (vq != 0) go to the *2 kernels, 0 (CKM_BLK=0): every model to the chunked ones
   // optional dense outputs for parity tests
   float *dense_filtersc, *dense_vit, *dense_fwd; uint8_t *dense_passed;
   const int32_t *model_slot; int32_t nseq;
 };
 int launch_bias(const FilterParams &p, int grid, cudaStream_t st);
 int launch_vit(const FilterParams &p, int grid, cudaStream_t st);
-// lane-block classes: class index c (0..9) keeps BLK_Q[c] model positions per lane; index 10 = the unblocked kernels
+// Lane-block classes.  A model of M <= 1024 positions gets vq = the smallest Q of BLK_Q with M <= 32 Q: its lane-blocked
+// kernels keep Q positions per lane (the packed Viterbi kernels W = Q/2 words), and from Q = 12 on the fp32 and int32
+// kernels hold the transitions in shared memory instead of registers (TSMEM).  Class index c (0..9) is the position of Q in
+// BLK_Q; index N_BLK_CLASSES = the unblocked (chunked) kernels, which also take every model with M > 1024 (vq = 0).
 constexpr int N_BLK_CLASSES = 10;
 constexpr int BLK_Q[N_BLK_CLASSES] = {2, 4, 6, 8, 12, 16, 20, 24, 28, 32};
+constexpr bool blk_tsmem(int q) { return q >= 12; }
+// the same table as arithmetic, usable in device code (the static_assert below holds it to BLK_Q)
+__host__ __device__ constexpr int vq_of(int M) { return M <= 256 ? 2 * ((M + 63) / 64) : M <= 1024 ? 4 * ((M + 127) / 128) : 0; }
+__host__ __device__ constexpr int blk_class(int vq) { return vq == 0 ? N_BLK_CLASSES : (vq <= 8 ? vq / 2 - 1 : vq / 4 + 1); }
+constexpr bool blk_table_ok(int c = 0) {
+  return c == N_BLK_CLASSES || (blk_class(BLK_Q[c]) == c && vq_of(32 * BLK_Q[c]) == BLK_Q[c] &&
+                                vq_of(32 * BLK_Q[c] + 1) == (c + 1 < N_BLK_CLASSES ? BLK_Q[c + 1] : 0) && blk_table_ok(c + 1));
+}
+static_assert(vq_of(1) == 2 && blk_table_ok(), "lane-block class arithmetic disagrees with BLK_Q");
+
+// f(Q, TSMEM) for class index cls, both as std::integral_constant; a class outside 0..9 is an error
+template <int C = 0, class F> int with_class(int cls, F &&f) {
+  if constexpr (C == N_BLK_CLASSES) {
+    set_error("bad lane-block class " + std::to_string(cls));
+    return CKM_EINVAL;
+  } else {
+    if (cls == C) return f(std::integral_constant<int, BLK_Q[C]>{}, std::integral_constant<bool, blk_tsmem(BLK_Q[C])>{});
+    return with_class<C + 1>(cls, f);
+  }
+}
+
+// one kernel launch: the dynamic shared-memory opt-in when smem is over 48 KB, the launch, the error check naming the kernel
+template <class... KA, class... A>
+int launch_kernel(void (*kern)(KA...), const char *name, int grid, int block, size_t smem, cudaStream_t st, const A &...args) {
+  cudaError_t e;
+  if (smem > 48 * 1024 && (e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess)
+    return cuda_fail(e, name);
+  kern<<<grid, block, smem, st>>>(args...);
+  e = cudaGetLastError();
+  return e == cudaSuccess ? CKM_OK : cuda_fail(e, name);
+}
+
 int launch_vit2(const FilterParams &p, int cls, int grid, cudaStream_t st);
 int launch_vitp(const FilterParams &p, int cls, int grid, cudaStream_t st);   // packed int16x2 kernels (kernels_vitp.cu)
 constexpr int VITP_CHUNK = 64;      // pairs of one model a packed-Viterbi CTA takes at a time
@@ -134,7 +170,7 @@ struct DomdefParams {
   const float *logsum_tbl;
   int32_t row_elems;
   const float4 *tfb; const float *rfb;   // lane-blocked tables
-  int32_t use_blk;                       // 1: models with a blocked class go to the *2 kernels
+  int32_t use_blk;                       // 1: models with a class (vq != 0) go to the *2 kernels, 0 (CKM_BLK=0): every model to the chunked ones
 };
 int launch_regions(const DomdefParams &p, int grid, cudaStream_t st);
 int launch_envelopes(const DomdefParams &p, int grid, cudaStream_t st);
