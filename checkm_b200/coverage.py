@@ -12,6 +12,7 @@ The coverage file's rows, their order and their text are the reference's at thre
 Differences from the reference, on purpose: a read that reaches the edit-distance test without an integer NM tag stops
 the run with the read's name (the reference's worker raises there and its contigs silently get 0), and the BAMs are
 walked in file order rather than by forked workers per contig."""
+import contextlib
 import logging
 import ntpath
 import os
@@ -38,6 +39,34 @@ class CoverageStruct():
 
 def batch_bytes():
     return int(float(os.environ.get('CKM_BAM_BATCH_MB', str(DEFAULT_BATCH_MB))) * (1 << 20))
+
+
+@contextlib.contextmanager
+def bam_batches(bamFile, timing):
+    """Opens bamFile's index, block table and header (bam.Layout) and yields (header, run).  run(call) sends every batch
+    through call(eng, comp, blocks, seg_start, seg_end, comp_base), one device call returning its inflate and scan ms.
+    Adds to `timing`: 'read' (opening), 'device_calls' (the rest), the kernel ms, the batches and their sizes."""
+    t0 = time.perf_counter()
+    lay = bam.Layout(bamFile)
+    t1 = time.perf_counter()
+
+    def run(call):
+        eng = runtime.engine()
+        for b0, b1, s, e in lay.batches(batch_bytes()):
+            comp, base = lay.comp(b0, b1)
+            ms_inf, ms_scan = call(eng, comp, lay.blocks[b0:b1], s, e, base)
+            timing['batches'] += 1
+            timing['inflate_ms'] += ms_inf
+            timing['scan_ms'] += ms_scan
+            timing['compressed_bytes'] += comp.size
+            timing['inflated_bytes'] += int(lay.U[b1] - lay.U[b0])
+            timing['segments'] += len(s)
+    try:
+        yield lay.header, run
+    finally:
+        timing['read'] += t1 - t0
+        timing['device_calls'] += time.perf_counter() - t1
+        lay.close()
 
 
 def print_summary(logger, cnt, numRefSeqs):
@@ -136,29 +165,13 @@ class Coverage():
     def _processBam(self, bamFile, bAllReads, minAlignPer, maxEditDistPer, minQC):
         """(names, lengths, n_ref x 9 int64 counters) of one BAM: reads, duplicates, secondary, failed QC, failed alignment
         length, failed edit distance, failed proper pair, mapped, aligned bases."""
-        t0 = time.perf_counter()
-        lay = bam.Layout(bamFile)
-        t1 = time.perf_counter()
-        try:
-            n_ref = len(lay.header.names)
+        with bam_batches(bamFile, self.timing) as (header, run):
+            n_ref = len(header.names)
             cnt = np.zeros((n_ref, 9), dtype=np.int64)
-            eng = runtime.engine()
-            for b0, b1, s, e in lay.batches(batch_bytes()):
-                comp, base = lay.comp(b0, b1)
-                ms_inf, ms_scan = eng.bam_coverage(comp, lay.blocks[b0:b1], s, e, n_ref, cnt, comp_base=base,
-                                                   all_reads=bAllReads, min_qc=minQC, min_align=minAlignPer,
-                                                   max_edit=maxEditDistPer)
-                self.timing['batches'] += 1
-                self.timing['inflate_ms'] += ms_inf
-                self.timing['scan_ms'] += ms_scan
-                self.timing['compressed_bytes'] += comp.size
-                self.timing['inflated_bytes'] += int(lay.U[b1] - lay.U[b0])
-                self.timing['segments'] += len(s)
-            return lay.header.names, lay.header.lengths, cnt
-        finally:
-            self.timing['read'] += t1 - t0
-            self.timing['device_calls'] += time.perf_counter() - t1
-            lay.close()
+            run(lambda eng, comp, blocks, s, e, base: eng.bam_coverage(
+                comp, blocks, s, e, n_ref, cnt, comp_base=base, all_reads=bAllReads, min_qc=minQC, min_align=minAlignPer,
+                max_edit=maxEditDistPer))
+            return header.names, header.lengths, cnt
 
     def _summary(self, cnt, numRefSeqs):
         """The per-BAM summary of coverage.py:258-287 (stdout), when the logger shows INFO."""

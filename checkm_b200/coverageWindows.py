@@ -24,16 +24,8 @@ import time
 
 import numpy as np
 
-from . import bam, runtime
 from ._lib import CkmError
-from .coverage import batch_bytes, print_summary
-
-
-class CoverageStruct():
-    def __init__(self, seqLen, mappedReads, coverage):
-        self.seqLen = seqLen
-        self.mappedReads = mappedReads
-        self.coverage = coverage
+from .coverage import CoverageStruct, bam_batches, print_summary  # noqa: F401 (CoverageStruct: the reference's name here)
 
 
 def window_offsets(lengths, windowSize):
@@ -90,29 +82,13 @@ class CoverageWindows():
 
     def _processBam(self, bamFile, bAllReads, minAlignPer, maxEditDistPer, windowSize):
         """(names, lengths, n_ref x 9 int64 counters, int64 window sums, window offsets) of one BAM."""
-        t0 = time.perf_counter()
-        lay = bam.Layout(bamFile)
-        t1 = time.perf_counter()
-        try:
-            names, lengths = lay.header.names, lay.header.lengths
+        with bam_batches(bamFile, self.timing) as (header, run):
+            names, lengths = header.names, header.lengths
             off = window_offsets(lengths, windowSize)
             cnt = np.zeros((len(names), 9), dtype=np.int64)
             win = np.zeros(int(off[-1]), dtype=np.int64)
             self.timing['windows'] = int(off[-1])
-            eng = runtime.engine()
-            for b0, b1, s, e in lay.batches(batch_bytes()):
-                comp, base = lay.comp(b0, b1)
-                ms_inf, ms_scan = eng.bam_windows(comp, lay.blocks[b0:b1], s, e, lengths, windowSize, off, cnt, win,
-                                                  comp_base=base, all_reads=bAllReads, min_align=minAlignPer,
-                                                  max_edit=maxEditDistPer)
-                self.timing['batches'] += 1
-                self.timing['inflate_ms'] += ms_inf
-                self.timing['scan_ms'] += ms_scan
-                self.timing['compressed_bytes'] += comp.size
-                self.timing['inflated_bytes'] += int(lay.U[b1] - lay.U[b0])
-                self.timing['segments'] += len(s)
+            run(lambda eng, comp, blocks, s, e, base: eng.bam_windows(
+                comp, blocks, s, e, lengths, windowSize, off, cnt, win, comp_base=base, all_reads=bAllReads,
+                min_align=minAlignPer, max_edit=maxEditDistPer))
             return names, lengths, cnt, win, off
-        finally:
-            self.timing['read'] += t1 - t0
-            self.timing['device_calls'] += time.perf_counter() - t1
-            lay.close()

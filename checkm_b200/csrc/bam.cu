@@ -1,5 +1,5 @@
-// bam.cu -- `checkm coverage` (checkm/coverage.py:57-287): BGZF blocks inflated on the device, BAM records walked and
-// classified on the device, nine integer counters per reference.
+// bam.cu -- `checkm coverage` (checkm/coverage.py:57-287) and `checkm gc_bias_plot`'s read depth per window: BGZF blocks
+// inflated on the device, BAM records walked and classified on the device, nine integer counters per reference.
 //
 // Layout.  The caller hands over one batch: the compressed bytes of consecutive BGZF blocks, their table (file offset,
 // length, ISIZE; ckm_bgzf_blocks) and the record segments to walk.  Block b inflates to out[U[b] .. U[b] + ISIZE[b]),
@@ -17,21 +17,23 @@
 //                        against ISIZE; a malformed block sets its status and the first bad block's index.  Last, each
 //                        lane takes the CRC32 of one slice of the output and lane 0 joins the 32 partial CRCs with the
 //                        shift operators x^(8n) mod P (zlib's crc32_combine), compared with the block's CRC field.
-//   bam_scan_kernel      one thread per segment [anchor_i, anchor_i+1): walks the records, validates each, classifies it
-//                        as coverage.py:206-230 does and keeps the counters in registers while refID stays the same;
-//                        they go out with 64-bit atomics when it changes.  A walk must land exactly on the segment's
-//                        end.  The first segment starts at the end of the header, so by induction every anchor (a
-//                        record start taken from the BAI's linear index) and every record start is verified; an index
-//                        that belongs to another file, or a truncated file, gives CKM_EFORMAT, never a wrong table.
-//                        The walk stops at the first record with refID -1 (the unplaced tail).
-//   bam_window_kernel    `checkm gc_bias_plot`'s read depth (coverageWindows.py:55-79): the same segments, the same record
-//                        decode, bounds checks and NM look-up, but coverageWindows' classification and the fetch rule of
-//                        `fetch(ref, 0, len)`.  Each mapped read adds its clipped span [pos, min(pos + alen, len)) to its
-//                        reference's covered bases and each window's overlap with it to an int64 window array.  The
-//                        thread keeps one (window, partial sum) in registers and flushes it with a 64-bit atomic when the
-//                        window changes; the reads are coordinate-sorted, so most reads land in the cached window.  Walkers
-//                        of neighbouring segments may share a window (segments end on 16 kbp index windows, not on W), and
-//                        the atomics make that correct.
+//   The record walk      one thread per segment [anchor_i, anchor_i+1) (`walk`, shared by the two kernels below): walks the
+//                        records, validates each, hands it to the kernel's rule to classify, and keeps the counters in
+//                        registers while refID stays the same; they go out with 64-bit atomics when it changes.  A walk
+//                        must land exactly on the segment's end.  The first segment starts at the end of the header, so
+//                        by induction every anchor (a record start taken from the BAI's linear index) and every record
+//                        start is verified; an index that belongs to another file, or a truncated file, gives
+//                        CKM_EFORMAT, never a wrong table.  The walk stops at the first record with refID -1 (the
+//                        unplaced tail).
+//   bam_scan_kernel      the walk with coverage.py:206-230's classification (CoverageRule).
+//   bam_window_kernel    the walk with `checkm gc_bias_plot`'s read depth (coverageWindows.py:55-79, WindowRule):
+//                        coverageWindows' classification and the fetch rule of `fetch(ref, 0, len)`.  Each mapped read
+//                        adds its clipped span [pos, min(pos + alen, len)) to its reference's covered bases and each
+//                        window's overlap with it to an int64 window array.  The thread keeps one (window, partial sum) in
+//                        registers and flushes it with a 64-bit atomic when the window changes; the reads are
+//                        coordinate-sorted, so most reads land in the cached window.  Walkers of neighbouring segments
+//                        may share a window (segments end on 16 kbp index windows, not on W), and the atomics make that
+//                        correct.
 #include <algorithm>
 #include <cstdint>
 #include <cstdio>
@@ -350,10 +352,11 @@ const char *scan_msg(int c) {
 // codes whose message names the read
 bool scan_names_read(int c) { return c == SC_NO_NM || c == SC_NO_NUM_NM || c == SC_NO_CIGAR || c == SC_NEG_POS; }
 
-struct ScanParams {
+// the parameters of both walk kernels
+struct WalkParams {
   const uint8_t *data;                        // 4-byte aligned, readable 8 bytes past the last segment end
   const int64_t *seg_start, *seg_end; int64_t nseg;
-  int32_t n_ref, all_reads, min_qc; double min_align, max_edit;
+  int32_t n_ref; ckm_bam_filter filter;
   unsigned long long *counters;               // n_ref x NCNT
   unsigned long long *err;                    // min of (record position << 8 | code)
 };
@@ -505,7 +508,14 @@ __device__ __forceinline__ void flush(unsigned long long *counters, int ref, uns
   for (int k = 0; k < NCNT; ++k) c[k] = 0;
 }
 
-__global__ void __launch_bounds__(SCAN_THREADS) bam_scan_kernel(ScanParams q) {
+// The walk of one segment by one thread, shared by both kernels.  The counters stay in registers while refID is the same
+// and are flushed when it changes; the walk ends at the segment's end, at the first unplaced record of the last segment,
+// or at the first record that stops it, whose position goes into the error word.  What a record counts for is the rule's:
+//   rule.reference(ref)     the walk enters reference ref (before its first record)
+//   rule.record(d, r, c)    classifies the decoded record r into c: SC_OK, or the code that stops the walk at r
+//   rule.finish()           after the final flush, whether or not the walk stopped early
+template <class Rule>
+__device__ __forceinline__ void walk(const WalkParams &q, Rule &rule) {
   const int64_t s = (int64_t)blockIdx.x * SCAN_THREADS + threadIdx.x;
   if (s >= q.nseg) return;
   const uint8_t *d = q.data;
@@ -517,44 +527,57 @@ __global__ void __launch_bounds__(SCAN_THREADS) bam_scan_kernel(ScanParams q) {
   int cur = -1, code = SC_OK;
   while (pos < end) {
     Rec r;
-    const int rc0 = decode_record(d, pos, end, q.n_ref, s == q.nseg - 1, r);
-    if (rc0) { if (rc0 != SC_TAIL) code = rc0; break; }
-    const int flag = r.flag, l_seq = r.l_seq;
-    if (r.ref != cur) { flush(q.counters, cur, c); cur = r.ref; }
-    c[0]++;
-    if (flag & 0x4) {
-    } else if (flag & 0x400) c[1]++;
-    else if (flag & 0x900) c[2]++;
-    else if ((flag & 0x200) || r.mapq < q.min_qc) c[3]++;
-    else {
-      const int64_t qal = aligned_length(d, r.cig, r.n_cigar, l_seq);
-      if ((double)qal < q.min_align * (double)l_seq) c[4]++;
-      else {
-        int64_t nm = 0;
-        const int rc = find_nm(d, r.aux, r.end, &nm);
-        if (rc) { code = rc; break; }
-        if ((double)nm > q.max_edit * (double)l_seq) c[5]++;
-        else if (!q.all_reads && !(flag & 0x2)) c[6]++;
-        else { c[7]++; c[8] += (unsigned long long)qal; }
-      }
-    }
+    const int rc = decode_record(d, pos, end, q.n_ref, s == q.nseg - 1, r);
+    if (rc) { if (rc != SC_TAIL) code = rc; break; }
+    if (r.ref != cur) { flush(q.counters, cur, c); cur = r.ref; rule.reference(cur); }
+    if ((code = rule.record(d, r, c))) break;
     pos = r.end;
   }
   if (code) atomicMin(q.err, (unsigned long long)pos << 8 | (unsigned long long)code);
   flush(q.counters, cur, c);
+  rule.finish();
+}
+
+// coverage.py:206-230
+struct CoverageRule {
+  const ckm_bam_filter &f;
+  __device__ void reference(int) {}
+  __device__ int record(const uint8_t *d, const Rec &r, unsigned long long *c) const {
+    const int flag = r.flag, l_seq = r.l_seq;
+    c[0]++;
+    if (flag & 0x4) {
+    } else if (flag & 0x400) c[1]++;
+    else if (flag & 0x900) c[2]++;
+    else if ((flag & 0x200) || r.mapq < f.min_qc) c[3]++;
+    else {
+      const int64_t qal = aligned_length(d, r.cig, r.n_cigar, l_seq);
+      if ((double)qal < f.min_align * (double)l_seq) c[4]++;
+      else {
+        int64_t nm = 0;
+        const int rc = find_nm(d, r.aux, r.end, &nm);
+        if (rc) return rc;
+        if ((double)nm > f.max_edit * (double)l_seq) c[5]++;
+        else if (!f.all_reads && !(flag & 0x2)) c[6]++;
+        else { c[7]++; c[8] += (unsigned long long)qal; }
+      }
+    }
+    return SC_OK;
+  }
+  __device__ void finish() {}
+};
+
+__global__ void __launch_bounds__(SCAN_THREADS) bam_scan_kernel(WalkParams q) {
+  CoverageRule rule{q.filter};
+  walk(q, rule);
 }
 
 struct WinParams {
-  const uint8_t *data;                        // as ScanParams
-  const int64_t *seg_start, *seg_end; int64_t nseg;
-  int32_t n_ref, all_reads; double min_align, max_edit;
+  WalkParams walk;                            // counters: the ninth is the clipped covered bases
   const int64_t *ref_len;                     // header lengths
   const int64_t *win_off;                     // n_ref + 1: reference r's windows are windows[win_off[r] .. win_off[r + 1])
   int64_t W;
-  unsigned long long *counters;               // n_ref x NCNT; the ninth is the clipped covered bases
   unsigned long long *windows;                // per window: the sum of the depth over it
   unsigned long long *touched;                // [0] smallest window written, [1] largest + 1
-  unsigned long long *err;
 };
 
 // reference span of the CIGAR: M, D, N, =, X (pysam's reference_length, coverageWindows' `alen`)
@@ -567,75 +590,67 @@ __device__ __forceinline__ int64_t reference_span(const uint8_t *d, int64_t cig,
   return s;
 }
 
-__global__ void __launch_bounds__(SCAN_THREADS) bam_window_kernel(WinParams q) {
-  const int64_t s = (int64_t)blockIdx.x * SCAN_THREADS + threadIdx.x;
-  if (s >= q.nseg) return;
-  const uint8_t *d = q.data;
-  int64_t pos = q.seg_start[s];
-  const int64_t end = q.seg_end[s];
-  unsigned long long c[NCNT];
-#pragma unroll
-  for (int k = 0; k < NCNT; ++k) c[k] = 0;
-  int cur = -1, code = SC_OK;
-  int64_t L = 0, off = 0, nwin = 0;
-  int64_t wi = -1;                                                 // cached window (global index) and its partial sum
+// coverageWindows.py:55-79 over the records fetch(ref, 0, L) yields
+struct WindowRule {
+  const WinParams &q;
+  int64_t L = 0, off = 0, nwin = 0;           // the current reference's length, first window and window count
+  int64_t wi = -1;                            // cached window (global index) and its partial sum
   unsigned long long wsum = 0;
-  unsigned long long lo = ~0ull, hi = 0;
-  const int64_t W = q.W;
-  while (pos < end) {
-    Rec r;
-    const int rc0 = decode_record(d, pos, end, q.n_ref, s == q.nseg - 1, r);
-    if (rc0) { if (rc0 != SC_TAIL) code = rc0; break; }
+  unsigned long long lo = ~0ull, hi = 0;      // the windows written: [lo, hi)
+  __device__ void reference(int ref) { L = q.ref_len[ref]; off = q.win_off[ref]; nwin = q.win_off[ref + 1] - off; }
+  __device__ int record(const uint8_t *d, const Rec &r, unsigned long long *c) {
+    const ckm_bam_filter &f = q.walk.filter;
+    const int64_t W = q.W;
     const int flag = r.flag;
     const double l_seq = (double)r.l_seq;
-    if (r.ref != cur) {
-      flush(q.counters, cur, c);
-      cur = r.ref; L = q.ref_len[cur]; off = q.win_off[cur]; nwin = q.win_off[cur + 1] - off;
-    }
     const int64_t alen = reference_span(d, r.cig, r.n_cigar);
     const int64_t rp = r.pos;
     // fetch(ref, 0, L) yields the records overlapping [0, L): end = pos + span, or pos + 1 when unmapped or empty
     const int64_t fend = rp + ((flag & 0x4) || alen == 0 ? 1 : alen);
-    if (rp < L && fend > 0) {
-      c[0]++;
-      if (flag & 0x4) {
-      } else if (flag & 0x400) c[1]++;
-      else if (flag & 0x100) c[2]++;                               // supplementary reads fall through
-      else if (flag & 0x200) c[3]++;                               // no mapping-quality threshold
-      else if (r.n_cigar == 0) { code = SC_NO_CIGAR; break; }
-      else if ((double)alen < q.min_align * l_seq) c[4]++;
+    if (rp >= L || fend <= 0) return SC_OK;
+    c[0]++;
+    if (flag & 0x4) {
+    } else if (flag & 0x400) c[1]++;
+    else if (flag & 0x100) c[2]++;                                 // supplementary reads fall through
+    else if (flag & 0x200) c[3]++;                                 // no mapping-quality threshold
+    else if (r.n_cigar == 0) return SC_NO_CIGAR;
+    else if ((double)alen < f.min_align * l_seq) c[4]++;
+    else {
+      double nm = 0.0;
+      const int rc = find_nm_number(d, r.aux, r.end, &nm);
+      if (rc) return rc;
+      if (nm > f.max_edit * l_seq) c[5]++;
+      else if (!f.all_reads && !(flag & 0x2)) c[6]++;
+      else if (rp < 0) return SC_NEG_POS;
       else {
-        double nm = 0.0;
-        const int rc = find_nm_number(d, r.aux, r.end, &nm);
-        if (rc) { code = rc; break; }
-        if (nm > q.max_edit * l_seq) c[5]++;
-        else if (!q.all_reads && !(flag & 0x2)) c[6]++;
-        else if (rp < 0) { code = SC_NEG_POS; break; }
-        else {
-          c[7]++;
-          const int64_t b = min(rp + alen, L);                     // numpy's slice clips at the reference end
-          if (b > rp) {
-            c[8] += (unsigned long long)(b - rp);
-            const int64_t klast = min((b - 1) / W, nwin - 1);
-            for (int64_t k = rp / W; k <= klast; ++k) {
-              const int64_t g = off + k;
-              if (g != wi) {
-                if (wsum) atomicAdd(q.windows + wi, wsum);
-                wi = g; wsum = 0;
-                lo = min(lo, (unsigned long long)g); hi = max(hi, (unsigned long long)g + 1);
-              }
-              wsum += (unsigned long long)(min(b, (k + 1) * W) - max(rp, k * W));
+        c[7]++;
+        const int64_t b = min(rp + alen, L);                       // numpy's slice clips at the reference end
+        if (b > rp) {
+          c[8] += (unsigned long long)(b - rp);
+          const int64_t klast = min((b - 1) / W, nwin - 1);
+          for (int64_t k = rp / W; k <= klast; ++k) {
+            const int64_t g = off + k;
+            if (g != wi) {
+              if (wsum) atomicAdd(q.windows + wi, wsum);
+              wi = g; wsum = 0;
+              lo = min(lo, (unsigned long long)g); hi = max(hi, (unsigned long long)g + 1);
             }
+            wsum += (unsigned long long)(min(b, (k + 1) * W) - max(rp, k * W));
           }
         }
       }
     }
-    pos = r.end;
+    return SC_OK;
   }
-  if (code) atomicMin(q.err, (unsigned long long)pos << 8 | (unsigned long long)code);
-  flush(q.counters, cur, c);
-  if (wsum) atomicAdd(q.windows + wi, wsum);
-  if (hi) { atomicMin(q.touched, lo); atomicMax(q.touched + 1, hi); }
+  __device__ void finish() {
+    if (wsum) atomicAdd(q.windows + wi, wsum);
+    if (hi) { atomicMin(q.touched, lo); atomicMax(q.touched + 1, hi); }
+  }
+};
+
+__global__ void __launch_bounds__(SCAN_THREADS) bam_window_kernel(WinParams q) {
+  WindowRule rule{q};
+  walk(q.walk, rule);
 }
 
 const uint32_t *x2n_table() {
@@ -739,28 +754,6 @@ int check_batch(const char *fn, int64_t comp_base, int64_t comp_len, const ckm_b
   return CKM_OK;
 }
 
-// Inflates the batch into dout and uploads the segments into dseg (starts, then ends).  kernel_ms_out[0]: the inflate.
-int inflate_and_upload(ckm_engine *e, const char *fn, const uint8_t *comp, int64_t comp_base, int64_t comp_len,
-                       const ckm_bgzf_block *blocks, int64_t nblocks, const std::vector<int64_t> &uoff,
-                       const int64_t *seg_start, const int64_t *seg_end, int64_t nseg, DevBuf &dout, DevBuf &dseg,
-                       float *kernel_ms_out, int64_t *err_offset_out) {
-  cudaStream_t st = e->stream;
-  int64_t bad_block = -1;
-  float ms_inflate = 0.0f;
-  int rc;
-  if ((rc = inflate_batch(e, fn, comp, comp_base, comp_len, blocks, nblocks, uoff, dout, &bad_block, &ms_inflate))) {
-    if (err_offset_out && bad_block >= 0) *err_offset_out = blocks[bad_block].coffset;
-    return rc;
-  }
-  if (kernel_ms_out) kernel_ms_out[0] = ms_inflate;
-  if ((rc = dseg.alloc(sizeof(int64_t) * 2 * (size_t)std::max<int64_t>(nseg, 1)))) return rc;
-  if (nseg) {
-    CKM_CUDA(cudaMemcpyAsync(dseg.p, seg_start, sizeof(int64_t) * (size_t)nseg, cudaMemcpyHostToDevice, st));
-    CKM_CUDA(cudaMemcpyAsync(dseg.as<int64_t>() + nseg, seg_end, sizeof(int64_t) * (size_t)nseg, cudaMemcpyHostToDevice, st));
-  }
-  return CKM_OK;
-}
-
 // CKM_EFORMAT for a walk's error word (record position << 8 | code): the record's virtual offset and, for the codes
 // that concern one read, its name.
 int scan_error(const char *fn, unsigned long long err, const ckm_bgzf_block *blocks, int64_t nblocks,
@@ -785,6 +778,72 @@ int scan_error(const char *fn, unsigned long long err, const ckm_bgzf_block *blo
   set_error(msg);
   if (err_offset_out) *err_offset_out = voff;
   return CKM_EFORMAT;
+}
+
+struct NoStep { int operator()() const { return CKM_OK; } };
+
+// One batch of ckm_bam_coverage or ckm_bam_windows (fn), from the argument check to the sum into `counters`: the batch
+// checks, the inflate, the segments, counters and error word on the device, the walk timed by events and its error.
+// launch(q, grid, st) launches the walk kernel with the shared parameters q.  prepare() runs after the batch checks and
+// before the inflate, in the same pool scope as the walk: the caller's own checks and buffers.  finish() runs after a
+// walk without error.
+template <class Launch, class Prepare = NoStep, class Finish = NoStep>
+int walk_batch(const char *fn, ckm_engine *e, const uint8_t *comp, int64_t comp_base, int64_t comp_len,
+               const ckm_bgzf_block *blocks, int64_t nblocks, const int64_t *seg_start, const int64_t *seg_end, int64_t nseg,
+               int32_t n_ref, const ckm_bam_filter *filter, int64_t *counters, float *kernel_ms_out, int64_t *err_offset_out,
+               Launch launch, Prepare prepare = Prepare(), Finish finish = Finish()) {
+  if (!e || comp_len < 0 || (comp_len > 0 && !comp) || nblocks < 0 || (nblocks > 0 && !blocks) || nseg < 0 ||
+      (nseg > 0 && (!seg_start || !seg_end)) || n_ref < 0 || !filter || (n_ref > 0 && !counters)) {
+    set_error(std::string(fn) + ": bad argument"); return CKM_EINVAL;
+  }
+  if (kernel_ms_out) kernel_ms_out[0] = kernel_ms_out[1] = 0.0f;
+  if (err_offset_out) *err_offset_out = -1;
+  std::vector<int64_t> uoff;
+  int rc;
+  if ((rc = check_batch(fn, comp_base, comp_len, blocks, nblocks, seg_start, seg_end, nseg, uoff))) return rc;
+  cudaSetDevice(e->device);
+  PoolScope pool_scope(e);
+  if ((rc = prepare())) return rc;
+  cudaStream_t st = e->stream;
+  DevBuf dout, dseg, dcnt, derr;
+  int64_t bad_block = -1;
+  float ms_inflate = 0.0f;
+  if ((rc = inflate_batch(e, fn, comp, comp_base, comp_len, blocks, nblocks, uoff, dout, &bad_block, &ms_inflate))) {
+    if (err_offset_out && bad_block >= 0) *err_offset_out = blocks[bad_block].coffset;
+    return rc;
+  }
+  if (kernel_ms_out) kernel_ms_out[0] = ms_inflate;
+  const size_t ncnt = (size_t)n_ref * NCNT;
+  if ((rc = dseg.alloc(sizeof(int64_t) * 2 * (size_t)std::max<int64_t>(nseg, 1))) ||
+      (rc = dcnt.alloc(sizeof(int64_t) * std::max<size_t>(ncnt, 1))) || (rc = derr.alloc(sizeof(unsigned long long))))
+    return rc;
+  if (nseg) {
+    CKM_CUDA(cudaMemcpyAsync(dseg.p, seg_start, sizeof(int64_t) * (size_t)nseg, cudaMemcpyHostToDevice, st));
+    CKM_CUDA(cudaMemcpyAsync(dseg.as<int64_t>() + nseg, seg_end, sizeof(int64_t) * (size_t)nseg, cudaMemcpyHostToDevice, st));
+  }
+  if (ncnt) CKM_CUDA(cudaMemsetAsync(dcnt.p, 0, sizeof(int64_t) * ncnt, st));
+  CKM_CUDA(cudaMemsetAsync(derr.p, 0xFF, sizeof(unsigned long long), st));
+  WalkParams q;
+  q.data = dout.as<uint8_t>(); q.seg_start = dseg.as<int64_t>(); q.seg_end = dseg.as<int64_t>() + nseg; q.nseg = nseg;
+  q.n_ref = n_ref; q.filter = *filter;
+  q.counters = dcnt.as<unsigned long long>(); q.err = derr.as<unsigned long long>();
+  CKM_CUDA(cudaEventRecord(e->ev[0], st));
+  if (nseg) {
+    launch(q, (unsigned)((nseg + SCAN_THREADS - 1) / SCAN_THREADS), st);
+    CKM_CUDA(cudaGetLastError());
+  }
+  CKM_CUDA(cudaEventRecord(e->ev[1], st));
+  unsigned long long err = 0;
+  std::vector<int64_t> cnt(ncnt);
+  CKM_CUDA(cudaMemcpyAsync(&err, derr.p, sizeof(err), cudaMemcpyDeviceToHost, st));
+  if (ncnt) CKM_CUDA(cudaMemcpyAsync(cnt.data(), dcnt.p, sizeof(int64_t) * ncnt, cudaMemcpyDeviceToHost, st));
+  CKM_CUDA(cudaStreamSynchronize(st));
+  float ms_scan = 0.0f;
+  CKM_CUDA(cudaEventElapsedTime(&ms_scan, e->ev[0], e->ev[1]));
+  if (kernel_ms_out) kernel_ms_out[1] = ms_scan;
+  if (err != ~0ull) return scan_error(fn, err, blocks, nblocks, uoff, dout, err_offset_out);
+  for (size_t k = 0; k < ncnt; ++k) counters[k] += cnt[k];
+  return finish();
 }
 
 }  // namespace
@@ -857,152 +916,86 @@ int ckm_bgzf_inflate(ckm_engine *e, const uint8_t *comp, int64_t comp_base, int6
 int ckm_bam_coverage(ckm_engine *e, const uint8_t *comp, int64_t comp_base, int64_t comp_len, const ckm_bgzf_block *blocks,
                      int64_t nblocks, const int64_t *seg_start, const int64_t *seg_end, int64_t nseg, int32_t n_ref,
                      const ckm_bam_filter *filter, int64_t *counters, float *kernel_ms_out, int64_t *err_offset_out) {
-  if (!e || comp_len < 0 || (comp_len > 0 && !comp) || nblocks < 0 || (nblocks > 0 && !blocks) || nseg < 0 ||
-      (nseg > 0 && (!seg_start || !seg_end)) || n_ref < 0 || !filter || (n_ref > 0 && !counters)) {
-    set_error("ckm_bam_coverage: bad argument"); return CKM_EINVAL;
-  }
-  if (kernel_ms_out) kernel_ms_out[0] = kernel_ms_out[1] = 0.0f;
-  if (err_offset_out) *err_offset_out = -1;
-  std::vector<int64_t> uoff;
-  int rc;
-  if ((rc = check_batch("ckm_bam_coverage", comp_base, comp_len, blocks, nblocks, seg_start, seg_end, nseg, uoff))) return rc;
-  cudaSetDevice(e->device);
-  PoolScope pool_scope(e);
-  cudaStream_t st = e->stream;
-  DevBuf dout, dseg;
-  if ((rc = inflate_and_upload(e, "ckm_bam_coverage", comp, comp_base, comp_len, blocks, nblocks, uoff, seg_start, seg_end, nseg,
-                               dout, dseg, kernel_ms_out, err_offset_out)))
-    return rc;
-  DevBuf dcnt, derr;
-  const size_t ncnt = (size_t)n_ref * NCNT;
-  if ((rc = dcnt.alloc(sizeof(int64_t) * std::max<size_t>(ncnt, 1))) || (rc = derr.alloc(sizeof(unsigned long long))))
-    return rc;
-  if (ncnt) CKM_CUDA(cudaMemsetAsync(dcnt.p, 0, sizeof(int64_t) * ncnt, st));
-  CKM_CUDA(cudaMemsetAsync(derr.p, 0xFF, sizeof(unsigned long long), st));
-  ScanParams q;
-  q.data = dout.as<uint8_t>(); q.seg_start = dseg.as<int64_t>(); q.seg_end = dseg.as<int64_t>() + nseg; q.nseg = nseg;
-  q.n_ref = n_ref; q.all_reads = filter->all_reads; q.min_qc = filter->min_qc;
-  q.min_align = filter->min_align; q.max_edit = filter->max_edit;
-  q.counters = dcnt.as<unsigned long long>(); q.err = derr.as<unsigned long long>();
-  CKM_CUDA(cudaEventRecord(e->ev[0], st));
-  if (nseg) {
-    bam_scan_kernel<<<(unsigned)((nseg + SCAN_THREADS - 1) / SCAN_THREADS), SCAN_THREADS, 0, st>>>(q);
-    CKM_CUDA(cudaGetLastError());
-  }
-  CKM_CUDA(cudaEventRecord(e->ev[1], st));
-  unsigned long long err = 0;
-  std::vector<int64_t> cnt(ncnt);
-  CKM_CUDA(cudaMemcpyAsync(&err, derr.p, sizeof(err), cudaMemcpyDeviceToHost, st));
-  if (ncnt) CKM_CUDA(cudaMemcpyAsync(cnt.data(), dcnt.p, sizeof(int64_t) * ncnt, cudaMemcpyDeviceToHost, st));
-  CKM_CUDA(cudaStreamSynchronize(st));
-  float ms_scan = 0.0f;
-  CKM_CUDA(cudaEventElapsedTime(&ms_scan, e->ev[0], e->ev[1]));
-  if (kernel_ms_out) kernel_ms_out[1] = ms_scan;
-  if (err != ~0ull) return scan_error("ckm_bam_coverage", err, blocks, nblocks, uoff, dout, err_offset_out);
-  for (size_t k = 0; k < ncnt; ++k) counters[k] += cnt[k];
-  return CKM_OK;
+  return walk_batch("ckm_bam_coverage", e, comp, comp_base, comp_len, blocks, nblocks, seg_start, seg_end, nseg, n_ref, filter,
+                    counters, kernel_ms_out, err_offset_out,
+                    [](const WalkParams &q, unsigned grid, cudaStream_t st) { bam_scan_kernel<<<grid, SCAN_THREADS, 0, st>>>(q); });
 }
 
 int ckm_bam_windows(ckm_engine *e, const uint8_t *comp, int64_t comp_base, int64_t comp_len, const ckm_bgzf_block *blocks,
                     int64_t nblocks, const int64_t *seg_start, const int64_t *seg_end, int64_t nseg, int32_t n_ref,
                     const ckm_bam_filter *filter, const int64_t *ref_len, int64_t window_size, const int64_t *win_off,
                     int64_t *counters, int64_t *windows, float *kernel_ms_out, int64_t *err_offset_out) {
-  if (!e || comp_len < 0 || (comp_len > 0 && !comp) || nblocks < 0 || (nblocks > 0 && !blocks) || nseg < 0 ||
-      (nseg > 0 && (!seg_start || !seg_end)) || n_ref < 0 || !filter || (n_ref > 0 && (!counters || !ref_len)) || !win_off) {
-    set_error("ckm_bam_windows: bad argument"); return CKM_EINVAL;
-  }
-  if (kernel_ms_out) kernel_ms_out[0] = kernel_ms_out[1] = 0.0f;
-  if (err_offset_out) *err_offset_out = -1;
-  char msg[320];
-  if (window_size <= 0) {
-    std::snprintf(msg, sizeof msg, "ckm_bam_windows: window size %lld; it must be at least 1", (long long)window_size);
-    set_error(msg); return CKM_EINVAL;
-  }
-  if (win_off[0] != 0) { set_error("ckm_bam_windows: win_off[0] must be 0"); return CKM_EINVAL; }
-  for (int32_t r = 0; r < n_ref; ++r) {
-    if (ref_len[r] <= 0) {
-      std::snprintf(msg, sizeof msg, "ckm_bam_windows: reference %d has length %lld; coverage per base needs a length of at "
-                    "least 1", r, (long long)ref_len[r]);
+  DevBuf dwin, dlen, dtouch;
+  auto prepare = [&]() -> int {
+    if ((n_ref > 0 && !ref_len) || !win_off) { set_error("ckm_bam_windows: bad argument"); return CKM_EINVAL; }
+    char msg[320];
+    if (window_size <= 0) {
+      std::snprintf(msg, sizeof msg, "ckm_bam_windows: window size %lld; it must be at least 1", (long long)window_size);
       set_error(msg); return CKM_EINVAL;
     }
-    if (win_off[r + 1] - win_off[r] != (ref_len[r] - 1) / window_size) {
-      std::snprintf(msg, sizeof msg, "ckm_bam_windows: reference %d has %lld windows in win_off, (length - 1) / window size "
-                    "is %lld", r, (long long)(win_off[r + 1] - win_off[r]), (long long)((ref_len[r] - 1) / window_size));
-      set_error(msg); return CKM_EINVAL;
+    if (win_off[0] != 0) { set_error("ckm_bam_windows: win_off[0] must be 0"); return CKM_EINVAL; }
+    for (int32_t r = 0; r < n_ref; ++r) {
+      if (ref_len[r] <= 0) {
+        std::snprintf(msg, sizeof msg, "ckm_bam_windows: reference %d has length %lld; coverage per base needs a length of at "
+                      "least 1", r, (long long)ref_len[r]);
+        set_error(msg); return CKM_EINVAL;
+      }
+      if (win_off[r + 1] - win_off[r] != (ref_len[r] - 1) / window_size) {
+        std::snprintf(msg, sizeof msg, "ckm_bam_windows: reference %d has %lld windows in win_off, (length - 1) / window size "
+                      "is %lld", r, (long long)(win_off[r + 1] - win_off[r]), (long long)((ref_len[r] - 1) / window_size));
+        set_error(msg); return CKM_EINVAL;
+      }
     }
-  }
-  const int64_t nwin = win_off[n_ref];
-  if (nwin > 0 && !windows) { set_error("ckm_bam_windows: bad argument"); return CKM_EINVAL; }
-  std::vector<int64_t> uoff;
-  int rc;
-  if ((rc = check_batch("ckm_bam_windows", comp_base, comp_len, blocks, nblocks, seg_start, seg_end, nseg, uoff))) return rc;
-  cudaSetDevice(e->device);
-  PoolScope pool_scope(e);
-  cudaStream_t st = e->stream;
-  // the window array first: it is the one buffer whose size the caller chooses through W
-  DevBuf dwin;
-  size_t free_b = 0, total_b = 0;
-  CKM_CUDA(cudaMemGetInfo(&free_b, &total_b));
-  const double need = 8.0 * (double)nwin;
-  if (need > (double)free_b || dwin.alloc(sizeof(int64_t) * (size_t)std::max<int64_t>(nwin, 1))) {
-    cudaGetLastError();
-    if (need <= (double)free_b) CKM_CUDA(cudaMemGetInfo(&free_b, &total_b));
-    // the smallest W whose window array fits in the free memory (sum of (len - 1) / W falls as W grows)
-    auto windows_at = [&](int64_t w) { int64_t t = 0; for (int32_t r = 0; r < n_ref; ++r) t += (ref_len[r] - 1) / w; return t; };
-    const int64_t cap = (int64_t)(free_b / 8);
-    int64_t lo_w = window_size, hi_w = window_size;
-    while (windows_at(hi_w) > cap && hi_w < (int64_t(1) << 40)) hi_w *= 2;
-    while (lo_w < hi_w) { const int64_t m = lo_w + (hi_w - lo_w) / 2; if (windows_at(m) > cap) lo_w = m + 1; else hi_w = m; }
-    std::snprintf(msg, sizeof msg, "ckm_bam_windows: %lld windows of %lld bp need %.1f MiB of device memory, %.1f MiB are "
-                  "free; the smallest window size that fits is %lld", (long long)nwin, (long long)window_size,
-                  need / 1048576.0, (double)free_b / 1048576.0, (long long)lo_w);
-    set_error(msg); return CKM_ENOMEM;
-  }
-  DevBuf dout, dseg;
-  if ((rc = inflate_and_upload(e, "ckm_bam_windows", comp, comp_base, comp_len, blocks, nblocks, uoff, seg_start, seg_end, nseg,
-                               dout, dseg, kernel_ms_out, err_offset_out)))
-    return rc;
-  DevBuf dcnt, dmeta, dlen;
-  const size_t ncnt = (size_t)n_ref * NCNT;
-  if ((rc = dcnt.alloc(sizeof(int64_t) * std::max<size_t>(ncnt, 1))) || (rc = dmeta.alloc(3 * sizeof(unsigned long long))) ||
-      (rc = dlen.alloc(sizeof(int64_t) * (2 * (size_t)n_ref + 1))))
-    return rc;
-  if (ncnt) CKM_CUDA(cudaMemsetAsync(dcnt.p, 0, sizeof(int64_t) * ncnt, st));
-  if (nwin) CKM_CUDA(cudaMemsetAsync(dwin.p, 0, sizeof(int64_t) * (size_t)nwin, st));
-  const unsigned long long meta0[3] = {~0ull, 0ull, ~0ull};        // touched [lo, hi), error
-  CKM_CUDA(cudaMemcpyAsync(dmeta.p, meta0, sizeof meta0, cudaMemcpyHostToDevice, st));
-  if (n_ref) CKM_CUDA(cudaMemcpyAsync(dlen.p, ref_len, sizeof(int64_t) * (size_t)n_ref, cudaMemcpyHostToDevice, st));
-  CKM_CUDA(cudaMemcpyAsync(dlen.as<int64_t>() + n_ref, win_off, sizeof(int64_t) * ((size_t)n_ref + 1), cudaMemcpyHostToDevice, st));
-  WinParams q;
-  q.data = dout.as<uint8_t>(); q.seg_start = dseg.as<int64_t>(); q.seg_end = dseg.as<int64_t>() + nseg; q.nseg = nseg;
-  q.n_ref = n_ref; q.all_reads = filter->all_reads; q.min_align = filter->min_align; q.max_edit = filter->max_edit;
-  q.ref_len = dlen.as<int64_t>(); q.win_off = dlen.as<int64_t>() + n_ref; q.W = window_size;
-  q.counters = dcnt.as<unsigned long long>(); q.windows = dwin.as<unsigned long long>();
-  q.touched = dmeta.as<unsigned long long>(); q.err = dmeta.as<unsigned long long>() + 2;
-  CKM_CUDA(cudaEventRecord(e->ev[0], st));
-  if (nseg) {
-    bam_window_kernel<<<(unsigned)((nseg + SCAN_THREADS - 1) / SCAN_THREADS), SCAN_THREADS, 0, st>>>(q);
-    CKM_CUDA(cudaGetLastError());
-  }
-  CKM_CUDA(cudaEventRecord(e->ev[1], st));
-  unsigned long long meta[3];
-  std::vector<int64_t> cnt(ncnt);
-  CKM_CUDA(cudaMemcpyAsync(meta, dmeta.p, sizeof meta, cudaMemcpyDeviceToHost, st));
-  if (ncnt) CKM_CUDA(cudaMemcpyAsync(cnt.data(), dcnt.p, sizeof(int64_t) * ncnt, cudaMemcpyDeviceToHost, st));
-  CKM_CUDA(cudaStreamSynchronize(st));
-  float ms_scan = 0.0f;
-  CKM_CUDA(cudaEventElapsedTime(&ms_scan, e->ev[0], e->ev[1]));
-  if (kernel_ms_out) kernel_ms_out[1] = ms_scan;
-  if (meta[2] != ~0ull) return scan_error("ckm_bam_windows", meta[2], blocks, nblocks, uoff, dout, err_offset_out);
-  for (size_t k = 0; k < ncnt; ++k) counters[k] += cnt[k];
+    const int64_t nwin = win_off[n_ref];
+    if (nwin > 0 && !windows) { set_error("ckm_bam_windows: bad argument"); return CKM_EINVAL; }
+    // the window array first: it is the one buffer whose size the caller chooses through W
+    size_t free_b = 0, total_b = 0;
+    CKM_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    const double need = 8.0 * (double)nwin;
+    if (need > (double)free_b || dwin.alloc(sizeof(int64_t) * (size_t)std::max<int64_t>(nwin, 1))) {
+      cudaGetLastError();
+      if (need <= (double)free_b) CKM_CUDA(cudaMemGetInfo(&free_b, &total_b));
+      // the smallest W whose window array fits in the free memory (sum of (len - 1) / W falls as W grows)
+      auto windows_at = [&](int64_t w) { int64_t t = 0; for (int32_t r = 0; r < n_ref; ++r) t += (ref_len[r] - 1) / w; return t; };
+      const int64_t cap = (int64_t)(free_b / 8);
+      int64_t lo_w = window_size, hi_w = window_size;
+      while (windows_at(hi_w) > cap && hi_w < (int64_t(1) << 40)) hi_w *= 2;
+      while (lo_w < hi_w) { const int64_t m = lo_w + (hi_w - lo_w) / 2; if (windows_at(m) > cap) lo_w = m + 1; else hi_w = m; }
+      std::snprintf(msg, sizeof msg, "ckm_bam_windows: %lld windows of %lld bp need %.1f MiB of device memory, %.1f MiB are "
+                    "free; the smallest window size that fits is %lld", (long long)nwin, (long long)window_size,
+                    need / 1048576.0, (double)free_b / 1048576.0, (long long)lo_w);
+      set_error(msg); return CKM_ENOMEM;
+    }
+    int rc;
+    if ((rc = dlen.alloc(sizeof(int64_t) * (2 * (size_t)n_ref + 1))) || (rc = dtouch.alloc(2 * sizeof(unsigned long long))))
+      return rc;
+    cudaStream_t st = e->stream;
+    if (nwin) CKM_CUDA(cudaMemsetAsync(dwin.p, 0, sizeof(int64_t) * (size_t)nwin, st));
+    const unsigned long long touched0[2] = {~0ull, 0ull};
+    CKM_CUDA(cudaMemcpyAsync(dtouch.p, touched0, sizeof touched0, cudaMemcpyHostToDevice, st));
+    if (n_ref) CKM_CUDA(cudaMemcpyAsync(dlen.p, ref_len, sizeof(int64_t) * (size_t)n_ref, cudaMemcpyHostToDevice, st));
+    CKM_CUDA(cudaMemcpyAsync(dlen.as<int64_t>() + n_ref, win_off, sizeof(int64_t) * ((size_t)n_ref + 1), cudaMemcpyHostToDevice, st));
+    return CKM_OK;
+  };
+  auto launch = [&](const WalkParams &w, unsigned grid, cudaStream_t st) {
+    const WinParams q{w, dlen.as<int64_t>(), dlen.as<int64_t>() + n_ref, window_size, dwin.as<unsigned long long>(),
+                      dtouch.as<unsigned long long>()};
+    bam_window_kernel<<<grid, SCAN_THREADS, 0, st>>>(q);
+  };
   // only the windows this batch wrote come back: a batch covers a run of references, not the whole array
-  if (meta[1] > meta[0]) {
-    const size_t lo = (size_t)meta[0], n = (size_t)(meta[1] - meta[0]);
-    std::vector<int64_t> w(n);
-    CKM_CUDA(cudaMemcpy(w.data(), dwin.as<int64_t>() + lo, sizeof(int64_t) * n, cudaMemcpyDeviceToHost));
-    for (size_t k = 0; k < n; ++k) windows[lo + k] += w[k];
-  }
-  return CKM_OK;
+  auto finish = [&]() -> int {
+    unsigned long long touched[2];
+    CKM_CUDA(cudaMemcpy(touched, dtouch.p, sizeof touched, cudaMemcpyDeviceToHost));
+    if (touched[1] > touched[0]) {
+      const size_t lo = (size_t)touched[0], n = (size_t)(touched[1] - touched[0]);
+      std::vector<int64_t> w(n);
+      CKM_CUDA(cudaMemcpy(w.data(), dwin.as<int64_t>() + lo, sizeof(int64_t) * n, cudaMemcpyDeviceToHost));
+      for (size_t k = 0; k < n; ++k) windows[lo + k] += w[k];
+    }
+    return CKM_OK;
+  };
+  return walk_batch("ckm_bam_windows", e, comp, comp_base, comp_len, blocks, nblocks, seg_start, seg_end, nseg, n_ref, filter,
+                    counters, kernel_ms_out, err_offset_out, launch, prepare, finish);
 }
 
 }  // extern "C"

@@ -96,6 +96,20 @@ class SeqDb:
             self._h = C.c_void_p()
 
 
+def _batch_args(fn, comp, blocks, comp_base, segs=(), counters=None, n_ref=0):
+    """The leading arguments of ckm_bgzf_inflate, ckm_bam_coverage and ckm_bam_windows for one BAM batch: comp, comp_base,
+    the block table, then the segments (seg_start, seg_end) if given; each pointer keeps its array alive through the call.
+    Given counters, checks them for the n_ref x 9 int64 sums the call adds to, in a message naming the method fn."""
+    comp = np.ascontiguousarray(np.frombuffer(comp, dtype=np.uint8) if not isinstance(comp, np.ndarray) else comp)
+    blocks = np.ascontiguousarray(blocks)
+    segs = [np.ascontiguousarray(x, dtype=np.int64) for x in segs]
+    if counters is not None and (counters.dtype != np.int64 or counters.shape != (n_ref, 9) or not counters.flags.c_contiguous):
+        raise ValueError(fn + ": counters must be a C-contiguous n_ref x 9 int64 array")
+    p = [a.ctypes.data_as(C.c_void_p) if a.size else None for a in [comp, blocks] + segs]
+    args = [p[0], int(comp_base), comp.size, p[1], len(blocks)]
+    return args + p[2:] + [len(segs[0])] if segs else args
+
+
 class Engine:
     """One engine per process per GPU (a CUDA context cannot cross fork())."""
 
@@ -280,33 +294,23 @@ class Engine:
     def bgzf_inflate(self, comp, blocks, comp_base=0):
         """The payloads of BGZF `blocks` (a bam.BLOCK_DTYPE table of file offsets; comp[0] is the byte at file offset
         comp_base) inflated back to back on the device (ckm_bgzf_inflate), and the inflate kernel's duration in ms."""
-        comp = np.ascontiguousarray(np.frombuffer(comp, dtype=np.uint8) if not isinstance(comp, np.ndarray) else comp)
-        blocks = np.ascontiguousarray(blocks)
-        total = int(blocks['isize'].sum())
+        batch = _batch_args('bgzf_inflate', comp, blocks, comp_base)
+        total = int(np.asarray(blocks)['isize'].sum())
         out = np.empty(max(total, 1), dtype=np.uint8)
         ms = C.c_float()
-        check(_lib.lib().ckm_bgzf_inflate(self._h, comp.ctypes.data if comp.size else None, int(comp_base), comp.size,
-                                          blocks.ctypes.data if len(blocks) else None, len(blocks), out.ctypes.data, out.size,
-                                          None, C.byref(ms)))
+        check(_lib.lib().ckm_bgzf_inflate(self._h, *batch, out.ctypes.data, out.size, None, C.byref(ms)))
         return out[:total], float(ms.value)
 
     def bam_coverage(self, comp, blocks, seg_start, seg_end, n_ref, counters, comp_base=0, all_reads=False, min_qc=15,
                      min_align=0.98, max_edit=0.02):
         """One batch of a BAM (ckm_bam_coverage): blocks inflated, the segments walked, the nine counters of every
         reference added to `counters` (n_ref x 9 int64).  Returns the inflate and scan kernels' durations in ms."""
-        comp = np.ascontiguousarray(np.frombuffer(comp, dtype=np.uint8) if not isinstance(comp, np.ndarray) else comp)
-        blocks = np.ascontiguousarray(blocks)
-        seg_start = np.ascontiguousarray(seg_start, dtype=np.int64)
-        seg_end = np.ascontiguousarray(seg_end, dtype=np.int64)
-        if counters.dtype != np.int64 or counters.shape != (n_ref, 9) or not counters.flags.c_contiguous:
-            raise ValueError("bam_coverage: counters must be a C-contiguous n_ref x 9 int64 array")
+        batch = _batch_args('bam_coverage', comp, blocks, comp_base, (seg_start, seg_end), counters, n_ref)
         filt = _lib.BamFilter(int(bool(all_reads)), int(min_qc), float(min_align), float(max_edit))
         ms = (C.c_float * 2)()
         err = C.c_int64()
-        check(_lib.lib().ckm_bam_coverage(self._h, comp.ctypes.data if comp.size else None, int(comp_base), comp.size,
-                                          blocks.ctypes.data if len(blocks) else None, len(blocks), seg_start.ctypes.data,
-                                          seg_end.ctypes.data, len(seg_start), int(n_ref), C.byref(filt),
-                                          counters.ctypes.data if n_ref else None, ms, C.byref(err)))
+        check(_lib.lib().ckm_bam_coverage(self._h, *batch, int(n_ref), C.byref(filt), counters.ctypes.data if n_ref else None,
+                                          ms, C.byref(err)))
         return float(ms[0]), float(ms[1])
 
     def bam_windows(self, comp, blocks, seg_start, seg_end, ref_len, window_size, win_off, counters, windows, comp_base=0,
@@ -315,15 +319,10 @@ class Engine:
         counters of every reference added to `counters` (n_ref x 9 int64; the ninth is the covered bases) and each
         window's depth sum to `windows` (int64; reference r owns windows[win_off[r]:win_off[r + 1]]).  Returns the
         inflate and window kernels' durations in ms."""
-        comp = np.ascontiguousarray(np.frombuffer(comp, dtype=np.uint8) if not isinstance(comp, np.ndarray) else comp)
-        blocks = np.ascontiguousarray(blocks)
-        seg_start = np.ascontiguousarray(seg_start, dtype=np.int64)
-        seg_end = np.ascontiguousarray(seg_end, dtype=np.int64)
         ref_len = np.ascontiguousarray(ref_len, dtype=np.int64)
         win_off = np.ascontiguousarray(win_off, dtype=np.int64)
         n_ref = len(ref_len)
-        if counters.dtype != np.int64 or counters.shape != (n_ref, 9) or not counters.flags.c_contiguous:
-            raise ValueError("bam_windows: counters must be a C-contiguous n_ref x 9 int64 array")
+        batch = _batch_args('bam_windows', comp, blocks, comp_base, (seg_start, seg_end), counters, n_ref)
         if win_off.shape != (n_ref + 1,):
             raise ValueError("bam_windows: win_off must hold n_ref + 1 offsets")
         if windows.dtype != np.int64 or windows.ndim != 1 or not windows.flags.c_contiguous or windows.size < win_off[-1]:
@@ -331,12 +330,9 @@ class Engine:
         filt = _lib.BamFilter(int(bool(all_reads)), 0, float(min_align), float(max_edit))
         ms = (C.c_float * 2)()
         err = C.c_int64()
-        check(_lib.lib().ckm_bam_windows(self._h, comp.ctypes.data if comp.size else None, int(comp_base), comp.size,
-                                         blocks.ctypes.data if len(blocks) else None, len(blocks), seg_start.ctypes.data,
-                                         seg_end.ctypes.data, len(seg_start), n_ref, C.byref(filt),
-                                         ref_len.ctypes.data if n_ref else None, int(window_size), win_off.ctypes.data,
-                                         counters.ctypes.data if n_ref else None, windows.ctypes.data if windows.size else None,
-                                         ms, C.byref(err)))
+        check(_lib.lib().ckm_bam_windows(self._h, *batch, n_ref, C.byref(filt), ref_len.ctypes.data if n_ref else None,
+                                         int(window_size), win_off.ctypes.data, counters.ctypes.data if n_ref else None,
+                                         windows.ctypes.data if windows.size else None, ms, C.byref(err)))
         return float(ms[0]), float(ms[1])
 
     def close(self):
