@@ -106,12 +106,14 @@ def _seq_stats(sc, seqStats=None):
 
 
 class _GeneFeatures(object):
-    """The three things bin statistics take from Prodigal's GFF (prodigal.py:202-273): the translation table, and per
-    sequence the number of bases covered by at least one gene."""
+    """What bin statistics and the plots take from Prodigal's GFF (prodigal.py:202-273): the translation table, per
+    sequence the number of bases covered by at least one gene, and per sequence the coding-base mask as disjoint intervals
+    (`intervals`, for `windowCodingBases`)."""
 
     def __init__(self, filename):
         self.translationTable = None
         genes, counter = {}, 0
+        self.lastCodingBase = {}                  # the largest gene end of every line of the sequence (overwritten genes too)
         for line in open(filename):
             if line.startswith('# Model Data') and not self.translationTable:
                 for token in line.split(';'):
@@ -125,6 +127,7 @@ class _GeneFeatures(object):
                 counter = 0                       # the running gene number restarts with every sequence first seen
                 genes[seqId] = {}
             genes[seqId][counter] = (int(fields[3]), int(fields[4]))
+            self.lastCodingBase[seqId] = max(self.lastCodingBase.get(seqId, 0), int(fields[4]))
             counter += 1
         self._covered = {}
         for seqId, spans in genes.items():
@@ -135,9 +138,42 @@ class _GeneFeatures(object):
                     covered += end - max(start - 1, reach)
                     reach = end
             self._covered[seqId] = covered
+        self.intervals = {seqId: self._mask_intervals(spans.values(), self.lastCodingBase[seqId]) for seqId, spans in genes.items()}
+
+    @staticmethod
+    def _mask_intervals(spans, L):
+        """prodigal.py:250-261: a mask of length L (the largest gene end) with mask[start-1:end] = 1 per gene, Python slice
+        semantics (a start of 0 marks only the last base; a start past L marks nothing), as sorted disjoint [lo, hi) and the
+        covered bases before each interval."""
+        cut = [slice(s - 1, e).indices(L)[:2] for s, e in spans]
+        merged = []
+        for lo, hi in sorted(c for c in cut if c[1] > c[0]):
+            if merged and lo <= merged[-1][1]:
+                merged[-1][1] = max(merged[-1][1], hi)
+            else:
+                merged.append([lo, hi])
+        lo = np.array([m[0] for m in merged], dtype=np.int64)
+        hi = np.array([m[1] for m in merged], dtype=np.int64)
+        before = np.concatenate([[0], np.cumsum(hi - lo)[:-1]]).astype(np.int64) if len(merged) else lo
+        return lo, hi, before
 
     def codingBases(self, seqId):
         return float(self._covered.get(seqId, 0))
+
+    def windowCodingBases(self, seqId, starts, ends):
+        """Per window [start, end) of the sequence: the number of mask positions set in it, np.sum(mask[start:end]) of
+        prodigal.py:263-273 (clipped to the mask; 0 for a sequence without a gene).  starts, ends: non-negative."""
+        starts = np.asarray(starts, dtype=np.int64)
+        ends = np.asarray(ends, dtype=np.int64)
+        if seqId not in self.intervals:
+            return np.zeros(len(starts), dtype=np.int64)
+        lo, hi, before = self.intervals[seqId]
+
+        def covered_below(pos):
+            j = np.searchsorted(lo, pos, side='right') - 1
+            jj = np.maximum(j, 0)
+            return np.where(j >= 0, before[jj] + np.minimum(pos, hi[jj]) - lo[jj], 0) if len(lo) else np.zeros(len(pos), dtype=np.int64)
+        return np.maximum(covered_below(ends) - covered_below(starts), 0)
 
 
 class BinStatistics(object):

@@ -12,10 +12,7 @@
 // CD table and the TD table; the sequence is outlying in GC when deltaGC < lower or deltaGC > upper, in CD when
 // deltaCD < lower, in TD when TD > upper (all strict; a nan compares false).
 //
-// np.sum and np.mean of a contiguous float64 vector add in numpy's pairwise order, not left to right: below 8 elements a
-// loop from 0.0; up to 128 elements eight running sums r[j] += a[i+j] combined as ((r0+r1)+(r2+r3))+((r4+r5)+(r6+r7)), the
-// tail added one by one; above 128 the vector is halved, the first half rounded down to a multiple of 8, and the halves'
-// sums added.  oracle/outliers_oracle.py states the same and tests/test_outliers_cpu.py holds it to the installed numpy.
+// np.sum and np.mean of a contiguous float64 vector add in numpy's pairwise order, not left to right (pairwise.cuh).
 //
 // Which GC and CD table a bin uses, and which percentile columns, depends on the bin means (binTools.py:250-261).  The
 // caller resolves that on the host from the same integer totals and passes each distinct (table, percentile columns) once as
@@ -39,11 +36,11 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
-#include <set>
 #include <thread>
 #include <vector>
 #include "engine.hpp"
 #include "pool.hpp"
+#include "pairwise.cuh"
 
 using namespace ckm;
 
@@ -56,7 +53,6 @@ struct ckm_sigs {
 namespace {
 
 constexpr int OL_COLS = 136;                   // canonical tetranucleotides
-constexpr int OL_LEAF = 128;                   // numpy's PW_BLOCKSIZE
 constexpr int OL_SEQ_VALUES = 9;               // GC, deltaGC, CD, deltaCD, TD, GC lower, GC upper, CD lower, TD upper
 constexpr int OL_AHEAD = 8;                    // signature rows in flight per column chain
 
@@ -160,31 +156,11 @@ __global__ void __launch_bounds__(256) outlier_seq_kernel(OutlierParams q) {
 __device__ __forceinline__ bool ol_node(long long n, int depth, unsigned slot, long long &off, long long &cnt) {
   off = 0; cnt = n;
   for (int d = depth - 1; d >= 0; --d) {
-    if (cnt <= OL_LEAF) return false;
-    long long n2 = cnt / 2;
-    n2 -= n2 % 8;
+    if (cnt <= PW_LEAF) return false;
+    const long long n2 = pw_split(cnt);
     if ((slot >> d) & 1u) { off += n2; cnt -= n2; } else cnt = n2;
   }
   return true;
-}
-
-__device__ double ol_leaf_sum(const double *a, int n) {
-  if (n < 8) {
-    double res = 0.0;
-    for (int i = 0; i < n; ++i) res += a[i];
-    return res;
-  }
-  double r[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) r[j] = a[j];
-  int i = 8;
-  for (; i < n - n % 8; i += 8) {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) r[j] += a[i + j];
-  }
-  double res = ((r[0] + r[1]) + (r[2] + r[3])) + ((r[4] + r[5]) + (r[6] + r[7]));
-  for (; i < n; ++i) res += a[i];
-  return res;
 }
 
 __global__ void __launch_bounds__(256) outlier_mean_kernel(OutlierParams q) {
@@ -197,32 +173,21 @@ __global__ void __launch_bounds__(256) outlier_mean_kernel(OutlierParams q) {
   for (unsigned i = threadIdx.x; i < slots; i += blockDim.x) {
     const int d = 31 - __clz(i + 1);
     long long off, cnt;
-    if (ol_node(n, d, i + 1 - (1u << d), off, cnt) && cnt <= OL_LEAF) heap[i] = ol_leaf_sum(a + off, (int)cnt);
+    if (ol_node(n, d, i + 1 - (1u << d), off, cnt) && cnt <= PW_LEAF) {
+      const double *leaf = a + off;
+      heap[i] = pw_leaf_sum([leaf](int k) { return leaf[k]; }, (int)cnt);
+    }
   }
   for (int d = D - 1; d >= 0; --d) {
     __syncthreads();
     for (unsigned slot = threadIdx.x; slot < (1u << d); slot += blockDim.x) {
       const unsigned i = (1u << d) - 1u + slot;
       long long off, cnt;
-      if (ol_node(n, d, slot, off, cnt) && cnt > OL_LEAF) heap[i] = heap[2 * i + 1] + heap[2 * i + 2];
+      if (ol_node(n, d, slot, off, cnt) && cnt > PW_LEAF) heap[i] = heap[2 * i + 1] + heap[2 * i + 2];
     }
   }
   __syncthreads();
   if (threadIdx.x == 0) q.means[3 * b + 2] = heap[0] / (double)n;
-}
-
-// depth of numpy's pairwise tree over n elements
-int pairwise_depth(long long n) {
-  std::set<long long> level{n};
-  int depth = 0;
-  for (;;) {
-    std::set<long long> next;
-    for (long long c : level)
-      if (c > OL_LEAF) { long long n2 = c / 2; n2 -= n2 % 8; next.insert(n2); next.insert(c - n2); }
-    if (next.empty()) return depth;
-    level.swap(next);
-    ++depth;
-  }
 }
 
 // one line `id\tv1\t...\tvN` of the profile file; returns 0, or the 1-based column that does not parse (ncols + 2: too many)

@@ -291,6 +291,32 @@ class Engine:
         check(_lib.lib().ckm_outlier_scores(self._h, sigs._h, C.byref(arg), C.byref(out)))
         return means, binsig, values, mask, tuple(float(v) for v in out.kernel_ms)
 
+    def window_stats(self, data, starts, lens, window_size, win_off, bin_sig=None):
+        """Per-window statistics of sequences laid out as `seqio.scan_nt_fasta` returns them (ckm_window_stats; sequence s
+        owns windows win_off[s]:win_off[s + 1], coverageWindows.window_offsets).  Returns the A, C, G, T(+U) counts of every
+        window (nwin x 4 int64), the tetranucleotide distance of every window to `bin_sig` (nwin float64, or None without
+        a signature) and the kernels' duration in ms."""
+        data = np.ascontiguousarray(data, dtype=np.uint8)
+        starts = np.ascontiguousarray(starts, dtype=np.int64)
+        lens = np.ascontiguousarray(lens, dtype=np.int64)
+        win_off = np.ascontiguousarray(win_off, dtype=np.int64)
+        if win_off.shape != (len(lens) + 1,):
+            raise ValueError("window_stats: win_off must hold one offset per sequence and one more")
+        nwin = int(win_off[-1])
+        acgt = np.zeros((nwin, 4), dtype=np.int64)
+        td = None
+        if bin_sig is not None:
+            bin_sig = np.ascontiguousarray(bin_sig, dtype=np.float64)
+            if bin_sig.shape != (136,):
+                raise ValueError("window_stats: bin_sig must hold 136 values")
+            td = np.zeros(nwin, dtype=np.float64)
+        ms = C.c_float()
+        check(_lib.lib().ckm_window_stats(self._h, data.ctypes.data if data.size else None, data.size, starts.ctypes.data,
+                                          lens.ctypes.data, len(lens), int(window_size), win_off.ctypes.data,
+                                          None if bin_sig is None else bin_sig.ctypes.data, acgt.ctypes.data,
+                                          None if td is None else td.ctypes.data, C.byref(ms)))
+        return acgt, td, float(ms.value)
+
     def bgzf_inflate(self, comp, blocks, comp_base=0):
         """The payloads of BGZF `blocks` (a bam.BLOCK_DTYPE table of file offsets; comp[0] is the byte at file offset
         comp_base) inflated back to back on the device (ckm_bgzf_inflate), and the inflate kernel's duration in ms."""

@@ -401,6 +401,18 @@ int  ckm_bam_windows(ckm_engine *e, const uint8_t *comp, int64_t comp_base, int6
                      const ckm_bam_filter *filter, const int64_t *ref_len, int64_t window_size, const int64_t *win_off,
                      int64_t *counters, int64_t *windows, float *kernel_ms_out, int64_t *err_offset_out);
 
+/* ---- plot windows (`checkm gc_plot`, `coding_plot`, `tetra_plot`, `dist_plot`, `gc_bias_plot`; checkm/plot/*.py): the
+ * statistics of every window of a bin's sequences in one device pass.  The arithmetic is stated in csrc/windows.cu. ---- */
+/* Sequences in the layout of ckm_fasta_scan_nt (same checks as ckm_scaffold_stats).  Window k of sequence s covers
+ * [k W, (k + 1) W) of it and exists only while (k + 1) W < length, so s owns windows win_off[s] .. win_off[s + 1], and
+ * win_off[s + 1] - win_off[s] must be (length - 1) / W (CKM_EINVAL otherwise, and for W < 1).  acgt_out (win_off[nseq] x 4):
+ * the A, C, G, T(+U) counts of every window, case-insensitive.  bin_sig (136 float64, optional): then td_out (win_off[nseq])
+ * receives each window's tetranucleotide distance np.sum(np.abs(sig - bin_sig)), sig its canonical 4-mer frequencies
+ * (NaN when no 4-mer of the window counts).  kernel_ms_out (optional): the kernels' duration by CUDA events. */
+int  ckm_window_stats(ckm_engine *e, const uint8_t *bytes, int64_t nbytes, const int64_t *starts, const int64_t *lens,
+                      int32_t nseq, int64_t window_size, const int64_t *win_off, const double *bin_sig, int64_t *acgt_out,
+                      double *td_out, float *kernel_ms_out);
+
 #ifdef __cplusplus
 }
 #endif
