@@ -88,7 +88,8 @@ SYMBOLS = ["ckm_init", "ckm_destroy", "ckm_last_error", "ckm_version", "ckm_devi
            "ckm_nccl_comm_init", "ckm_nccl_comm_destroy", "ckm_fasta_scan_nt", "ckm_scaffold_stats",
            "ckm_kmer_counts", "ckm_kmer_columns", "ckm_format_kmer_profiles", "ckm_merge_pairs", "ckm_format_merger_rows",
            "ckm_bgzf_blocks", "ckm_bgzf_inflate", "ckm_bam_coverage", "ckm_bam_windows",
-           "ckm_parse_kmer_profiles", "ckm_sigs_create", "ckm_sigs_free", "ckm_outlier_scores", "ckm_window_stats"]
+           "ckm_parse_kmer_profiles", "ckm_sigs_create", "ckm_sigs_free", "ckm_outlier_scores", "ckm_window_stats",
+           "ckm_id_join", "ckm_format_unbinned"]
 
 _lib = None
 
@@ -130,6 +131,9 @@ def lib():
     L.ckm_sigs_free.argtypes = [vp]
     L.ckm_sigs_free.restype = None
     L.ckm_outlier_scores.argtypes = [vp, vp, C.POINTER(OutlierIn), C.POINTER(OutlierOut)]
+    L.ckm_id_join.argtypes = [vp, C.c_char_p, i64, i32, vp, i64, vp, vp, vp, vp, vp, C.POINTER(i64), C.POINTER(i64),
+                              C.POINTER(C.c_float)]
+    L.ckm_format_unbinned.argtypes = [vp, vp, vp, vp, vp, vp, vp, i64, vp, i64, vp, i64, C.POINTER(i64), C.POINTER(i64)]
     L.ckm_window_stats.argtypes = [vp, vp, i64, vp, vp, i32, i64, vp, vp, vp, vp, C.POINTER(C.c_float)]
     L.ckm_bgzf_blocks.argtypes = [vp, i64, i64, vp, i64, C.POINTER(i64), C.POINTER(i64)]
     L.ckm_bgzf_inflate.argtypes = [vp, vp, i64, i64, vp, i64, vp, i64, C.POINTER(i64), C.POINTER(C.c_float)]

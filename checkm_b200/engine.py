@@ -291,6 +291,30 @@ class Engine:
         check(_lib.lib().ckm_outlier_scores(self._h, sigs._h, C.byref(arg), C.byref(out)))
         return means, binsig, values, mask, tuple(float(v) for v in out.kernel_ms)
 
+    def id_join(self, text, bin_nrec, nasm):
+        """The ids of the bins' and the assembly's records joined in one device call (ckm_id_join).  text: every header
+        line followed by '\\n', the bins' (bin_nrec[b] per file) before the assembly's (nasm).  Returns id_start, id_len
+        (per record, int64, byte spans in text), asm_flags (uint8: 1 = binned id, 2 = first record of its id), asm_last
+        (int64: the last assembly record of its id), bin_keep (bool: the last record of its id in its own bin file), the
+        number of distinct binned ids and the kernels' duration in ms.  A header without an id raises CkmError with the
+        record's index as its `record` attribute (-1 for every other error)."""
+        bin_nrec = np.ascontiguousarray(bin_nrec, dtype=np.int64)
+        n = int(bin_nrec.sum()) + int(nasm)
+        id_start = np.zeros(n, dtype=np.int64)
+        id_len = np.zeros(n, dtype=np.int64)
+        flags = np.zeros(nasm, dtype=np.uint8)
+        last = np.zeros(nasm, dtype=np.int32)
+        keep = np.zeros(n - nasm, dtype=np.uint8)
+        nbinned, bad, ms = C.c_int64(), C.c_int64(), C.c_float()
+        rc = _lib.lib().ckm_id_join(self._h, text, len(text), len(bin_nrec), bin_nrec.ctypes.data, int(nasm),
+                                    id_start.ctypes.data, id_len.ctypes.data, flags.ctypes.data, last.ctypes.data,
+                                    keep.ctypes.data, C.byref(nbinned), C.byref(bad), C.byref(ms))
+        if rc:
+            err = _lib.CkmError(rc, _lib.lib().ckm_last_error().decode(errors="replace"))
+            err.record = int(bad.value)
+            raise err
+        return id_start, id_len, flags, last.astype(np.int64), keep.view(bool), int(nbinned.value), float(ms.value)
+
     def window_stats(self, data, starts, lens, window_size, win_off, bin_sig=None):
         """Per-window statistics of sequences laid out as `seqio.scan_nt_fasta` returns them (ckm_window_stats; sequence s
         owns windows win_off[s]:win_off[s + 1], coverageWindows.window_offsets).  Returns the A, C, G, T(+U) counts of every

@@ -43,10 +43,9 @@ def read_bytes(path):
         return f.read()
 
 
-def scan_nt_fasta(raw):
-    """A nucleotide FASTA file as the reference's readFasta sees it (checkm/util/seqUtils.py:180-211), laid out for the
-    device scan: returns ids (first token of each header line), the byte buffer, and the start (a multiple of 64) and
-    length of every record.  A record whose id repeats replaces the earlier one, as in the reference's dict."""
+def scan_nt_raw(raw):
+    """ckm_fasta_scan_nt on one file's bytes: the header lines (text after '>', joined by '\\n', as bytes), the byte
+    buffer, and the start (a multiple of 64) and length of every record, repeated ids included."""
     n = len(raw)
     max_rec = int(np.count_nonzero(np.frombuffer(raw, dtype=np.uint8) == 62))     # '>' bytes: an upper bound on the records
     data = np.empty(n + 64 * (max_rec + 1), dtype=np.uint8)
@@ -57,14 +56,22 @@ def scan_nt_fasta(raw):
     _lib.check(_lib.lib().ckm_fasta_scan_nt(raw, n, data.ctypes.data, data.size, starts.ctypes.data, lens.ctypes.data, max_rec,
                                             headers, max(n, 1), C.byref(nrec), C.byref(used), C.byref(hb)))
     k = nrec.value
+    return headers.raw[:hb.value], data[:used.value], starts[:k], lens[:k]
+
+
+def scan_nt_fasta(raw):
+    """A nucleotide FASTA file as the reference's readFasta sees it (checkm/util/seqUtils.py:180-211), laid out for the
+    device scan: returns ids (first token of each header line), the byte buffer, and the start (a multiple of 64) and
+    length of every record.  A record whose id repeats replaces the earlier one, as in the reference's dict."""
+    hdr, data, starts, lens = scan_nt_raw(raw)
+    k = len(lens)
     if k == 0:
-        return [], data[:0], starts[:0], lens[:0]
-    ids = [line.split(None, 1)[0] for line in headers.raw[:hb.value].decode('utf-8', 'replace').split('\n')]   # IndexError: header without an id
-    starts, lens = starts[:k], lens[:k]
+        return [], data[:0], starts, lens
+    ids = [line.split(None, 1)[0] for line in hdr.decode('utf-8', 'replace').split('\n')]   # IndexError: header without an id
     if len(set(ids)) != k:
         last = {}
         for i, name in enumerate(ids):
             last[name] = i                             # dict order = first appearance, content = last appearance
         keep = np.array(list(last.values()), dtype=np.int64)
         ids, starts, lens = list(last.keys()), starts[keep], lens[keep]
-    return ids, data[:used.value], starts, lens
+    return ids, data, starts, lens

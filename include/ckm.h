@@ -413,6 +413,28 @@ int  ckm_window_stats(ckm_engine *e, const uint8_t *bytes, int64_t nbytes, const
                       int32_t nseq, int64_t window_size, const int64_t *win_off, const double *bin_sig, int64_t *acgt_out,
                       double *td_out, float *kernel_ms_out);
 
+/* ---- unbinned sequences (`checkm unbinned`; checkm/unbinned.py:33-85, util/seqUtils.py:180-211): the ids of the bins'
+ * records and of the assembly's joined in one device pass (csrc/idjoin.cu states how). ---- */
+/* text: one header line per record (the text after '>', as ckm_fasta_scan_nt returns them), each followed by '\n': the
+ * records of bin file 0, 1, ... (bin_nrec[b] each), then the nasm records of the assembly; UTF-8.  A record's id is
+ * line.split(None, 1)[0] (whitespace = Python's str.isspace()); ids are equal iff their bytes are.  Per record (bins'
+ * first): id_start_out / id_len_out, the id's bytes in text.  Per assembly record a: asm_flags_out[a] bit 0 = its id occurs
+ * in a bin, bit 1 = a is the first assembly record with its id (the dict's entries, in dict order); asm_last_out[a] = the
+ * last assembly record with its id (the dict's content).  Per bin record: bin_keep_out = it is the last record of its id in
+ * its own file.  *n_binned_ids_out: the ids that occur in any bin.  A header line without an id: CKM_EFORMAT and
+ * *bad_record_out = that record's index (the first such), -1 otherwise.  kernel_ms_out (optional): the kernels' duration
+ * by CUDA events. */
+int  ckm_id_join(ckm_engine *e, const char *text, int64_t nbytes, int32_t nbins, const int64_t *bin_nrec, int64_t nasm,
+                 int64_t *id_start_out, int64_t *id_len_out, uint8_t *asm_flags_out, int32_t *asm_last_out,
+                 uint8_t *bin_keep_out, int64_t *n_binned_ids_out, int64_t *bad_record_out, float *kernel_ms_out);
+/* host only: for each of n records, ">id\nsequence\n" into fasta_out and "id\tlength\t%.2f\n" into stats_out, the value
+ * float(g + c) * 100 / (a + c + g + t) in IEEE double from acgt (n x 4: A, C, G, T+U; a zero sum -> CKM_EINVAL).  Ids:
+ * ids[id_start[r] .. + id_len[r]); sequences: bytes[starts[r] .. + lens[r]).  *fasta_len_out / *stats_len_out: the bytes
+ * written, or, with CKM_ECAPACITY, bounds on the bytes needed. */
+int  ckm_format_unbinned(const char *ids, const int64_t *id_start, const int64_t *id_len, const uint8_t *bytes,
+                         const int64_t *starts, const int64_t *lens, const int64_t *acgt, int64_t n, char *fasta_out,
+                         int64_t fasta_cap, char *stats_out, int64_t stats_cap, int64_t *fasta_len_out, int64_t *stats_len_out);
+
 #ifdef __cplusplus
 }
 #endif
