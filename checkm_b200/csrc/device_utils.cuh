@@ -13,6 +13,16 @@ __device__ __forceinline__ uint4 lds128(uint32_t addr) {
   asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
   return v;
 }
+__device__ __forceinline__ uint32_t lds32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr));
+  return v;
+}
+__device__ __forceinline__ uint32_t lds8(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(addr));
+  return v;
+}
 
 // prmt.b32 with the PTX selector semantics (bit 3 of a selector nibble replicates the sign of the selected byte; the
 // __byte_perm intrinsic masks that bit off)

@@ -10,7 +10,7 @@
 // byte; the K-1 bytes it needs from before its row are in the 16-byte halo staged in front of the row, so warps never
 // join anything.  Per row a warp takes four 512-byte blocks, a lane 16 consecutive bytes of each (one conflict-free
 // LDS.128); the codes of the three bytes before a lane's 16 come from the lane before it by one shuffle.  Bases are
-// encoded with the low-three-bit PRMT lookup of ntstats (A 1, C 3, T 4, G 7 -> 2-bit codes A 0, C 1, G 2, T 3), and every
+// encoded with the low-three-bit PRMT lookup of ntrows.cuh (A 1, C 3, T 4, G 7 -> 2-bit codes A 0, C 1, G 2, T 3), and every
 // valid window adds one to a per-warp histogram over the 4^K raw window codes in shared memory (one ATOMS per window).
 // At the last row of a sequence, and at the end of the warp's range, the histogram is folded onto the canonical columns
 // (column c = code x plus its reverse complement) and written: by plain stores when the warp saw the whole sequence,
@@ -33,9 +33,7 @@ namespace {
 constexpr int KM_THREADS = 256;
 constexpr int KM_WARPS = KM_THREADS / 32;
 constexpr int KM_STAGES = 3;                                   // rows in flight per warp
-constexpr int KM_DESC_OFF = KM_STAGES * NT_STAGE;              // per-warp shared memory: stages, descriptors, mbarriers, histogram
-constexpr int KM_BAR_OFF = KM_DESC_OFF + KM_STAGES * 16;
-constexpr int KM_HIST_OFF = (KM_BAR_OFF + KM_STAGES * 8 + 127) / 128 * 128;
+constexpr int KM_HIST_OFF = (NtRing<KM_STAGES>::SMEM + 127) / 128 * 128;   // per-warp shared memory: the ring, the histogram
 constexpr int KM_WARP_SMEM = KM_HIST_OFF + 256 * 4;            // 7.4 KB per warp, 59 KB per CTA
 constexpr int KM_CTAS_PER_SM = 3;
 constexpr int KM_MAX_COLS = 136;
@@ -49,19 +47,6 @@ struct KmParams {
 
 __host__ __device__ constexpr int km_cols(int k) { return k == 1 ? 2 : k == 2 ? 10 : k == 3 ? 32 : 136; }
 
-// reverse complement of a K-mer code (2 bits per base, the last base lowest; A 0, C 1, G 2, T 3 so complement = xor 3)
-__host__ __device__ __forceinline__ uint32_t km_revcomp(uint32_t x, int k) {
-  uint32_t r = 0;
-  for (int i = 0; i < k; ++i) { r = (r << 2) | ((x & 3u) ^ 3u); x >>= 2; }
-  return r;
-}
-
-__device__ __forceinline__ uint32_t lds32(uint32_t addr) {
-  uint32_t v;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr));
-  return v;
-}
-
 // 0x80 in every byte of x that is zero
 __device__ __forceinline__ uint32_t zero4(uint32_t x) {
   const uint32_t t = (x & 0x7F7F7F7Fu) + 0x7F7F7F7Fu;
@@ -71,10 +56,8 @@ __device__ __forceinline__ uint32_t zero4(uint32_t x) {
 // One word of 4 bytes -> (valid nibble << 8) | packed codes: byte 0 (the earliest) in the top bits of both, so that
 // appending a word to earlier codes is a shift by 8 (codes) or 4 (valid bits).  keep: bytes of the word in the sequence.
 __device__ __forceinline__ uint32_t km_encode(uint32_t w, uint32_t keep) {
-  uint32_t t = w & 0x07070707u;
-  t |= t >> 4;
-  const uint32_t sel = prmt_b32(t, 0u, 0x4420);                  // the four 3-bit indices as selector nibbles
-  const uint32_t bad = (w & 0xDFDFDFDFu) ^ prmt_b32(0x43FF41FFu, 0x47FFFF54u, sel);   // 'a' -> 'A'; 0 where the byte is ACGTacgt
+  const uint32_t sel = nt_sel(w);
+  const uint32_t bad = (w & 0xDFDFDFDFu) ^ nt_letters(sel);                           // 'a' -> 'A'; 0 where the byte is ACGTacgt
   const uint32_t codes = prmt_b32(0x01000000u, 0x02000003u, sel);                     // A 0, C 1, G 2, T 3 per byte
   const uint32_t packed = (codes * 0x40100401u) >> 24;                                // byte b -> bits 6-2b, 7-2b
   const uint32_t valid = ((((zero4(bad) >> 7) * 0x08040201u) >> 24) & 0xFu) & ((0xFu << (4u - keep)) & 0xFu);   // byte b -> bit 3-b
@@ -91,32 +74,16 @@ __global__ void __launch_bounds__(KM_THREADS, KM_CTAS_PER_SM) kmer_kernel(KmPara
   for (int i = threadIdx.x; i < C; i += KM_THREADS) s_col[i] = p.col_code[i];
   __syncthreads();
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const long long gw = (long long)blockIdx.x * KM_WARPS + warp, nw = (long long)gridDim.x * KM_WARPS;
-  const long long lo = p.nrows * gw / nw, hi = p.nrows * (gw + 1) / nw;
-  if (lo >= hi) return;
-  const int n = (int)(hi - lo);
-  const NtRow *mine = p.rows + lo;
-  const uint32_t ring = smem_u32(s_dyn) + warp * KM_WARP_SMEM;
+  const NtRange r = nt_warp_rows(p.nrows, (long long)blockIdx.x * KM_WARPS + warp, (long long)gridDim.x * KM_WARPS);
+  if (r.lo >= r.hi) return;
+  NtRing<KM_STAGES> ring(smem_u32(s_dyn) + warp * KM_WARP_SMEM, p.rows + r.lo, (int)(r.hi - r.lo), lane);
   uint32_t *hist = reinterpret_cast<uint32_t *>(s_dyn + warp * KM_WARP_SMEM + KM_HIST_OFF);
   for (int i = lane; i < NBINS; i += 32) hist[i] = 0u;
-  NtRow upcoming = {0, 0u, 0u};
-  if (lane == 0) {
-    for (int i = 0; i < KM_STAGES; ++i) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(ring + KM_BAR_OFF + i * 8) : "memory");
-    fence_mbar_init();
-    for (int i = 0; i < KM_STAGES && i < n; ++i) nt_issue(mine[i], ring + i * NT_STAGE, ring + KM_DESC_OFF + i * 16, ring + KM_BAR_OFF + i * 8);
-    if (KM_STAGES < n) upcoming = mine[KM_STAGES];
-  }
-  __syncwarp();
-  int st = 0; uint32_t phase = 0;
+  ring.start();
   bool whole = false;                                            // the warp saw the first row of the sequence now open
-  for (int k = 0; k < n; ++k) {
-    nt_wait(ring + KM_BAR_OFF + st * 8, phase);
-    const uint4 d = lds128(ring + KM_DESC_OFF + st * 16);
-    const uint32_t s = d.z;
-    const int nbytes = (int)(d.w & 0xFFFu);
-    const bool first_row = (d.w >> 30) & 1u, last_row = (d.w >> 31) != 0;
+  for (int k = 0; k < ring.n; ++k) {
+    const auto [src, s, nbytes, first_row, last_row, body] = ring.wait();
     if (k == 0 || first_row) whole = first_row;
-    const uint32_t body = ring + st * NT_STAGE + NT_HALO;
     // the three bytes before the row: the halo, except at a sequence's first row (whatever is there is not sequence)
     uint32_t carry = 0;
     if (lane == 0 && !first_row) carry = km_encode(lds32(body - 4), 4u);
@@ -125,11 +92,7 @@ __global__ void __launch_bounds__(KM_THREADS, KM_CTAS_PER_SM) kmer_kernel(KmPara
     for (int q = 0; q < 4; ++q) v[q] = lds128(body + q * 512 + lane * 16);
     // every value read from the stage is in registers: it can take the row KM_STAGES further on
     __syncwarp();
-    if (lane == 0 && k + KM_STAGES < n) {
-      nt_issue(upcoming, ring + st * NT_STAGE, ring + KM_DESC_OFF + st * 16, ring + KM_BAR_OFF + st * 8);
-      if (k + KM_STAGES + 1 < n) upcoming = mine[k + KM_STAGES + 1];
-    }
-    if (++st == KM_STAGES) { st = 0; phase ^= 1u; }
+    ring.release(k);
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
       const int at = q * 512 + lane * 16;                        // where the lane's 16 bytes sit in the row
@@ -154,7 +117,7 @@ __global__ void __launch_bounds__(KM_THREADS, KM_CTAS_PER_SM) kmer_kernel(KmPara
         prev = e[j];
       }
     }
-    if (last_row || k + 1 == n) {
+    if (last_row || k + 1 == ring.n) {
       __syncwarp();
       uint32_t *out = p.counts + (size_t)s * C;
 #pragma unroll
@@ -177,14 +140,6 @@ __global__ void __launch_bounds__(KM_THREADS, KM_CTAS_PER_SM) kmer_kernel(KmPara
 }  // namespace
 
 namespace {
-
-// The columns of K: canonical k-mer codes in ascending order (= lexicographic order of the strings, A < C < G < T).
-int km_col_codes(int k, uint8_t *out) {
-  int c = 0;
-  for (uint32_t x = 0; x < (1u << (2 * k)); ++x)
-    if (x <= km_revcomp(x, k)) out[c++] = (uint8_t)x;
-  return c;
-}
 
 // str(np.float64(v)) for 0 <= v <= 1 or NaN: the shortest round-trip digits, laid out as Python's float repr does
 // (positional for 1e-4 <= v < 1e16, else d.ddde-XX; '.0' after an integer).
@@ -225,40 +180,27 @@ int ckm_kmer_counts(ckm_engine *e, const uint8_t *bytes, int64_t nbytes, const i
   }
   if (kernel_ms_out) *kernel_ms_out = 0.0f;
   if (nseq == 0) return CKM_OK;
-  for (int32_t s = 0; s < nseq; ++s) {
-    if ((starts[s] & 63) || lens[s] < 0 || lens[s] > 0xFFFFFFFFll || starts[s] < 0 || (starts[s] + lens[s] + 63) / 64 * 64 > nbytes) {
-      set_error("ckm_kmer_counts: every sequence must start at a multiple of 64 bytes and lie, padded to 64, inside the buffer");
-      return CKM_EINVAL;
-    }
-  }
+  if (int rc = nt_check_layout("ckm_kmer_counts", "sequence", starts, lens, nseq, nbytes)) return rc;
   const int ncols = km_cols(k);
   const size_t out_bytes = sizeof(uint32_t) * (size_t)ncols * (size_t)nseq;
   cudaSetDevice(e->device);
   PoolScope pool_scope(e);
   cudaStream_t st = e->stream;
-  DevBuf dbytes;
-  { int rc0 = dbytes.alloc((size_t)nbytes + 64); if (rc0) return rc0; }
-  std::vector<NtRow> rows;
-  nt_build_rows(dbytes.as<uint8_t>(), starts, lens, nseq, nbytes, rows);
-  const int64_t nrows = (int64_t)rows.size();
-  if (nrows == 0) { std::memset(counts_out, 0, out_bytes); return CKM_OK; }
-  if (nrows > 0x7FFFFFFFll) { set_error("ckm_kmer_counts: too many bytes for one call"); return CKM_EINVAL; }
-  DevBuf drows, dcounts;
-  int rc;
-  if ((rc = drows.alloc(sizeof(NtRow) * nrows)) || (rc = dcounts.alloc(out_bytes))) return rc;
-  CKM_CUDA(cudaMemcpyAsync(dbytes.p, bytes, (size_t)nbytes, cudaMemcpyHostToDevice, st));
-  CKM_CUDA(cudaMemcpyAsync(drows.p, rows.data(), sizeof(NtRow) * nrows, cudaMemcpyHostToDevice, st));
+  const int dyn_smem = KM_WARPS * KM_WARP_SMEM;
+  void (*kern)(KmParams) = k == 1 ? kmer_kernel<1> : k == 2 ? kmer_kernel<2> : k == 3 ? kmer_kernel<3> : kmer_kernel<4>;
+  NtUpload u;
+  if (int rc = nt_upload(e, "ckm_kmer_counts", bytes, nbytes, starts, lens, nseq, (const void *)kern, KM_WARPS, KM_CTAS_PER_SM, dyn_smem, u))
+    return rc;
+  if (u.nrows == 0) { std::memset(counts_out, 0, out_bytes); return CKM_OK; }
+  DevBuf dcounts;
+  if (int rc = dcounts.alloc(out_bytes)) return rc;
   CKM_CUDA(cudaMemsetAsync(dcounts.p, 0, out_bytes, st));
   KmParams p;
   std::memset(&p, 0, sizeof(p));
-  p.rows = drows.as<NtRow>(); p.nrows = nrows; p.counts = dcounts.as<uint32_t>();
+  p.rows = u.rows.as<NtRow>(); p.nrows = u.nrows; p.counts = dcounts.as<uint32_t>();
   km_col_codes(k, p.col_code);
-  const int grid = (int)std::min<int64_t>((int64_t)e->prop.multiProcessorCount * KM_CTAS_PER_SM, (nrows + KM_WARPS - 1) / KM_WARPS);
-  const int dyn_smem = KM_WARPS * KM_WARP_SMEM;
-  void (*kern)(KmParams) = k == 1 ? kmer_kernel<1> : k == 2 ? kmer_kernel<2> : k == 3 ? kmer_kernel<3> : kmer_kernel<4>;
-  CKM_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn_smem));
   CKM_CUDA(cudaEventRecord(e->ev[0], st));
-  kern<<<grid, KM_THREADS, dyn_smem, st>>>(p);
+  kern<<<u.grid, KM_THREADS, dyn_smem, st>>>(p);
   CKM_CUDA(cudaGetLastError());
   CKM_CUDA(cudaEventRecord(e->ev[1], st));
   CKM_CUDA(cudaMemcpyAsync(counts_out, dcounts.p, out_bytes, cudaMemcpyDeviceToHost, st));

@@ -27,23 +27,18 @@ namespace {
 constexpr int NT_THREADS = 256;
 constexpr int NT_WARPS = NT_THREADS / 32;
 // NT_CHUNK (64 bytes of one lane: one bit each in a 64-bit mask), NT_ROW, NT_HALO (9 bytes before and 1 after a row are
-// looked at) and NT_STAGE: ntrows.cuh
+// looked at), NT_STAGE and the ring: ntrows.cuh
 constexpr int NT_STAGES = 3;                         // rows in flight per warp
-constexpr int NT_DESC_OFF = NT_STAGES * NT_STAGE;    // per-warp shared memory: the stages, their row descriptors, their mbarriers
-constexpr int NT_BAR_OFF = NT_DESC_OFF + NT_STAGES * 16;
-constexpr int NT_WARP_SMEM = (NT_BAR_OFF + NT_STAGES * 8 + 127) / 128 * 128;
-#ifndef CKM_NT_CTAS
-#define CKM_NT_CTAS 4
-#endif
-constexpr int NT_CTAS_PER_SM = CKM_NT_CTAS;          // 4: 32 warps x 3 x 2 KB of stages = 200 KB of shared memory, <= 64 registers
+constexpr int NT_WARP_SMEM = (NtRing<NT_STAGES>::SMEM + 127) / 128 * 128;
+constexpr int NT_CTAS_PER_SM = 4;                    // 32 warps x 3 x 2 KB of stages = 200 KB of shared memory, <= 64 registers
 
 // The scaffolds of a call, cut into 2 KB rows, form one list; every warp of the grid takes a contiguous range of it and
 // streams its rows through its own ring of shared-memory stages, filled by TMA bulk copies that lane 0 issues NT_STAGES
 // ahead.  Warps never wait for each other.  A "piece" is the part of one scaffold inside one warp's range.  Contigs closed
 // inside a piece are reported by the kernel; the bases before the first run end of a piece (head) and after its last (tail)
 // come back separately and the host joins tail + head across the cuts (ckm_scaffold_stats below).
-// Piece index = scaffold + warp: along the list one of the two grows at every cut.  The rows (NtRow) and the copies that
-// stage them (nt_issue, nt_wait): ntrows.cuh.
+// Piece index = scaffold + warp: along the list one of the two grows at every cut.  The rows (NtRow), the warp split
+// (nt_warp_rows) and the ring (NtRing): ntrows.cuh.
 struct NtPiece { uint32_t head, tail, closed, pad; };              // closed: the piece holds at least one run end
 
 struct NtParams {
@@ -79,34 +74,19 @@ __device__ __forceinline__ void nt_emit(const NtParams &p, uint32_t scaf, uint32
 __global__ void __launch_bounds__(NT_THREADS, NT_CTAS_PER_SM) ntstats_kernel(NtParams p) {
   extern __shared__ __align__(128) uint8_t s_dyn[];             // NT_WARPS x NT_WARP_SMEM
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const long long gw = (long long)blockIdx.x * NT_WARPS + warp, nw = (long long)gridDim.x * NT_WARPS;
-  const long long lo = p.nrows * gw / nw, hi = p.nrows * (gw + 1) / nw;
-  if (lo >= hi) return;
-  const int n = (int)(hi - lo);                                  // rows of this warp (the host keeps a call below 2^31 rows)
-  const NtRow *mine = p.rows + lo;
-  const uint32_t ring = smem_u32(s_dyn) + warp * NT_WARP_SMEM;     // stage i at ring + i * NT_STAGE
-  NtRow upcoming = {0, 0u, 0u};                                  // lane 0: the row to issue next, fetched one row early
-  if (lane == 0) {
-    for (int i = 0; i < NT_STAGES; ++i) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(ring + NT_BAR_OFF + i * 8) : "memory");
-    fence_mbar_init();
-    for (int i = 0; i < NT_STAGES && i < n; ++i) nt_issue(mine[i], ring + i * NT_STAGE, ring + NT_DESC_OFF + i * 16, ring + NT_BAR_OFF + i * 8);
-    if (NT_STAGES < n) upcoming = mine[NT_STAGES];
-  }
-  __syncwarp();
+  const long long gw = (long long)blockIdx.x * NT_WARPS + warp;
+  const NtRange r = nt_warp_rows(p.nrows, gw, (long long)gridDim.x * NT_WARPS);
+  if (r.lo >= r.hi) return;
+  NtRing<NT_STAGES> ring(smem_u32(s_dyn) + warp * NT_WARP_SMEM, p.rows + r.lo, (int)(r.hi - r.lo), lane);
+  ring.start();
   const int rot = (lane >> 1) & 3;                               // the lane reads its four 16-byte vectors starting at this one:
                                                                  // eight neighbouring lanes then touch eight different bank groups
   uint32_t cA = 0, cC = 0, cG = 0, cT = 0, cN = 0, cn = 0;       // per-lane counts over the piece
   uint32_t carry = 0;                                            // bases of the contig still open (same in every lane)
   uint32_t head = 0; bool closed = false;                        // same in every lane
-  int st = 0; uint32_t phase = 0;
   uint32_t tail9 = 0;                                            // lane 0: is-N of the nine bytes before the row
-  for (int k = 0; k < n; ++k) {
-    nt_wait(ring + NT_BAR_OFF + st * 8, phase);
-    const uint4 d = lds128(ring + NT_DESC_OFF + st * 16);
-    const uint32_t s = d.z;
-    const int nbytes = (int)(d.w & 0xFFFu);
-    const bool first_row = (d.w >> 30) & 1u, last_row = (d.w >> 31) != 0;
-    const uint32_t body = ring + st * NT_STAGE + NT_HALO;
+  for (int k = 0; k < ring.n; ++k) {
+    const auto [src, s, nbytes, first_row, last_row, body] = ring.wait();
     const int left = nbytes - lane * NT_CHUNK;                   // bytes of the scaffold in and after this lane's chunk
     uint32_t w[16];
 #pragma unroll
@@ -122,7 +102,7 @@ __global__ void __launch_bounds__(NT_THREADS, NT_CTAS_PER_SM) ntstats_kernel(NtP
       halo_bits = nibble(eq4(v.y, 0x4E4E4E4Eu)) | (nibble(eq4(v.z, 0x4E4E4E4Eu)) << 4) | (nibble(eq4(v.w, 0x4E4E4E4Eu)) << 8);
       tail9 = halo_bits >> 3;                                    // bytes -12..-1 -> the last nine
     }
-    if (lane == 31 && !last_row) halo_bits = s_dyn[warp * NT_WARP_SMEM + st * NT_STAGE + NT_HALO + NT_ROW] == 'N';
+    if (lane == 31 && !last_row) halo_bits = lds8(body + NT_ROW) == 'N';
 
     unsigned long long m = 0, valid = 0;
     if (left > 0) {
@@ -141,10 +121,8 @@ __global__ void __launch_bounds__(NT_THREADS, NT_CTAS_PER_SM) ntstats_kernel(NtP
       uint32_t bad = 0, cg0 = 0, cg1 = 0, tt = 0;
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
-        uint32_t t = w[j] & 0x07070707u;
-        t |= t >> 4;
-        const uint32_t sel = prmt_b32(t, 0u, 0x4420);           // the four 3-bit indices as selector nibbles (all below 8)
-        bad |= w[j] ^ prmt_b32(0x43FF41FFu, 0x47FFFF54u, sel);
+        const uint32_t sel = nt_sel(w[j]);
+        bad |= w[j] ^ nt_letters(sel);
         const uint32_t cg = prmt_b32(0x01000000u, 0x10000000u, sel);
         if (j < 8) cg0 += cg; else cg1 += cg;
         tt += prmt_b32(0u, 0x00000001u, sel);
@@ -227,13 +205,8 @@ __global__ void __launch_bounds__(NT_THREADS, NT_CTAS_PER_SM) ntstats_kernel(NtP
       closed = closed || th;
     }
     tail9 = __shfl_sync(0xffffffffu, (uint32_t)(m >> 55), 31);
-    // every value read from the stage has been used: it can take the row NT_STAGES further on
-    if (lane == 0 && k + NT_STAGES < n) {
-      nt_issue(upcoming, ring + st * NT_STAGE, ring + NT_DESC_OFF + st * 16, ring + NT_BAR_OFF + st * 8);
-      if (k + NT_STAGES + 1 < n) upcoming = mine[k + NT_STAGES + 1];
-    }
-    if (++st == NT_STAGES) { st = 0; phase ^= 1u; }
-    if (last_row || k + 1 == n) {
+    ring.release(k);                                             // every value read from the stage has been used
+    if (last_row || k + 1 == ring.n) {
       const uint32_t v[6] = {cA, cC, cG, cT, cN, cn};
 #pragma unroll
       for (int i = 0; i < 6; ++i) { const uint32_t x = __reduce_add_sync(0xffffffffu, v[i]); if (lane == i && x) atomicAdd(&p.stats[(size_t)s * 8 + i], (unsigned long long)x); }
@@ -308,46 +281,35 @@ int ckm_scaffold_stats(ckm_engine *e, const uint8_t *bytes, int64_t nbytes, cons
   *ncontigs_out = 0;
   if (kernel_ms_out) *kernel_ms_out = 0.0f;
   if (nscaf == 0) return CKM_OK;
-  for (int32_t s = 0; s < nscaf; ++s) {
-    if ((starts[s] & 63) || lens[s] < 0 || lens[s] > 0xFFFFFFFFll || starts[s] < 0 || (starts[s] + lens[s] + 63) / 64 * 64 > nbytes) {
-      set_error("ckm_scaffold_stats: every scaffold must start at a multiple of 64 bytes and lie, padded to 64, inside the buffer");
-      return CKM_EINVAL;
-    }
-  }
+  if (int rc = nt_check_layout("ckm_scaffold_stats", "scaffold", starts, lens, nscaf, nbytes)) return rc;
   cudaSetDevice(e->device);
   PoolScope pool_scope(e);
   cudaStream_t st = e->stream;
-  DevBuf dbytes;
-  { int rc0 = dbytes.alloc((size_t)nbytes + 64); if (rc0) return rc0; }
-  std::vector<NtRow> rows;
-  nt_build_rows(dbytes.as<uint8_t>(), starts, lens, nscaf, nbytes, rows);
-  const int64_t nrows = (int64_t)rows.size();
   std::memset(stats_out, 0, sizeof(int64_t) * 8 * nscaf);
+  const int dyn_smem = NT_WARPS * NT_WARP_SMEM;
+  NtUpload u;
+  if (int rc = nt_upload(e, "ckm_scaffold_stats", bytes, nbytes, starts, lens, nscaf, (const void *)ntstats_kernel, NT_WARPS,
+                         NT_CTAS_PER_SM, dyn_smem, u))
+    return rc;
+  const int64_t nrows = u.nrows;
   if (nrows == 0) return CKM_OK;
-  if (nrows > 0x7FFFFFFFll) { set_error("ckm_scaffold_stats: too many bytes for one call"); return CKM_EINVAL; }
-  const int grid = (int)std::min<int64_t>((int64_t)e->prop.multiProcessorCount * NT_CTAS_PER_SM, (nrows + NT_WARPS - 1) / NT_WARPS);
-  const int64_t nwarps = (int64_t)grid * NT_WARPS;
+  const int64_t nwarps = (int64_t)u.grid * NT_WARPS;
   const size_t npiece = (size_t)nscaf + nwarps;
-  DevBuf drows, dpiece, dstats, dcs, dcl, dctr;
+  DevBuf dpiece, dstats, dcs, dcl, dctr;
   int rc;
-  if ((rc = drows.alloc(sizeof(NtRow) * nrows)) || (rc = dpiece.alloc(sizeof(NtPiece) * npiece)) ||
-      (rc = dstats.alloc(sizeof(int64_t) * 8 * nscaf)) ||
+  if ((rc = dpiece.alloc(sizeof(NtPiece) * npiece)) || (rc = dstats.alloc(sizeof(int64_t) * 8 * nscaf)) ||
       (rc = dcs.alloc(sizeof(uint32_t) * (size_t)contig_cap)) || (rc = dcl.alloc(sizeof(uint32_t) * (size_t)contig_cap)) || (rc = dctr.alloc(64)))
     return rc;
-  CKM_CUDA(cudaMemcpyAsync(dbytes.p, bytes, (size_t)nbytes, cudaMemcpyHostToDevice, st));
-  CKM_CUDA(cudaMemcpyAsync(drows.p, rows.data(), sizeof(NtRow) * nrows, cudaMemcpyHostToDevice, st));
   CKM_CUDA(cudaMemsetAsync(dpiece.p, 0, sizeof(NtPiece) * npiece, st));
   CKM_CUDA(cudaMemsetAsync(dctr.p, 0, 64, st));
   CKM_CUDA(cudaMemsetAsync(dstats.p, 0, sizeof(int64_t) * 8 * nscaf, st));
   NtParams p;
-  p.bytes = dbytes.as<uint8_t>(); p.rows = drows.as<NtRow>(); p.nrows = nrows; p.piece = dpiece.as<NtPiece>();
+  p.bytes = u.bytes.as<uint8_t>(); p.rows = u.rows.as<NtRow>(); p.nrows = nrows; p.piece = dpiece.as<NtPiece>();
   p.stats = dstats.as<unsigned long long>();
   p.contig_scaf = dcs.as<uint32_t>(); p.contig_len = dcl.as<uint32_t>();
   p.ncontigs = reinterpret_cast<unsigned long long *>(dctr.as<uint8_t>() + 8); p.cap = contig_cap;
-  const int dyn_smem = NT_WARPS * NT_WARP_SMEM;
-  CKM_CUDA(cudaFuncSetAttribute(ntstats_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn_smem));
   CKM_CUDA(cudaEventRecord(e->ev[0], st));
-  ntstats_kernel<<<grid, NT_THREADS, dyn_smem, st>>>(p);
+  ntstats_kernel<<<u.grid, NT_THREADS, dyn_smem, st>>>(p);
   CKM_CUDA(cudaGetLastError());
   CKM_CUDA(cudaEventRecord(e->ev[1], st));
   unsigned long long n_dev = 0;
@@ -363,9 +325,9 @@ int ckm_scaffold_stats(ckm_engine *e, const uint8_t *bytes, int64_t nbytes, cons
   {
     int64_t cur = -1; uint64_t open = 0;
     for (int64_t c = 0; c < nwarps; ++c) {
-      const int64_t lo = nrows * c / nwarps, hi = nrows * (c + 1) / nwarps;
-      if (lo >= hi) continue;
-      for (int64_t s = rows[lo].scaf; s <= (int64_t)rows[hi - 1].scaf; ++s) {
+      const NtRange r = nt_warp_rows(nrows, c, nwarps);
+      if (r.lo >= r.hi) continue;
+      for (int64_t s = u.host_rows[r.lo].scaf; s <= (int64_t)u.host_rows[r.hi - 1].scaf; ++s) {
         if (lens[s] == 0) continue;
         if (s != cur) { if (open) joined.emplace_back((uint32_t)cur, (uint32_t)open); cur = s; open = 0; }
         const NtPiece &r = piece[(size_t)s + c];

@@ -45,9 +45,7 @@ constexpr int WN_THREADS = 256;
 constexpr int WN_WARPS = WN_THREADS / 32;
 constexpr int WN_STAGES = 3;                                   // rows in flight per warp
 constexpr int WN_COLS = 136;                                   // canonical tetranucleotides
-constexpr int WN_DESC_OFF = WN_STAGES * NT_STAGE;              // per-warp shared memory: stages, descriptors, mbarriers, histograms
-constexpr int WN_BAR_OFF = WN_DESC_OFF + WN_STAGES * 16;
-constexpr int WN_HIST_OFF = (WN_BAR_OFF + WN_STAGES * 8 + 15) / 16 * 16;
+constexpr int WN_HIST_OFF = NtRing<WN_STAGES>::SMEM;           // per-warp shared memory: the ring, the histograms
 constexpr int WN_WARP_SMEM = (WN_HIST_OFF + 2 * WN_COLS * 4 + 127) / 128 * 128;   // 7.4 KB per warp, 59 KB per CTA
 constexpr int WN_CTAS_PER_SM = 2;                             // 3 would cap the scan at 80 registers and spill
 
@@ -86,48 +84,27 @@ __global__ void __launch_bounds__(WN_THREADS, WN_CTAS_PER_SM) window_scan_kernel
   for (int i = threadIdx.x; i < 256; i += WN_THREADS) s_col[i] = p.col_of[i];
   __syncthreads();
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const long long gw = (long long)blockIdx.x * WN_WARPS + warp, nw = (long long)gridDim.x * WN_WARPS;
-  const long long lo = p.nrows * gw / nw, hi = p.nrows * (gw + 1) / nw;
-  if (lo >= hi) return;
-  const int n = (int)(hi - lo);
-  const NtRow *mine = p.rows + lo;
-  const uint32_t ring = smem_u32(s_dyn) + warp * WN_WARP_SMEM;
+  const NtRange r = nt_warp_rows(p.nrows, (long long)blockIdx.x * WN_WARPS + warp, (long long)gridDim.x * WN_WARPS);
+  if (r.lo >= r.hi) return;
+  NtRing<WN_STAGES> ring(smem_u32(s_dyn) + warp * WN_WARP_SMEM, p.rows + r.lo, (int)(r.hi - r.lo), lane);
   uint32_t *hist = reinterpret_cast<uint32_t *>(s_dyn + warp * WN_WARP_SMEM + WN_HIST_OFF);   // 2 x 136
   for (int i = lane; i < 2 * WN_COLS; i += 32) hist[i] = 0u;
   long long hk0 = -1, hk1 = -1;                                  // window of each histogram slot (same in every lane)
   const long long W = p.W;
   const bool shared_hist = p.kmers != nullptr && W >= NT_ROW;
-  NtRow upcoming = {0, 0u, 0u};
-  if (lane == 0) {
-    for (int i = 0; i < WN_STAGES; ++i) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(ring + WN_BAR_OFF + i * 8) : "memory");
-    fence_mbar_init();
-    for (int i = 0; i < WN_STAGES && i < n; ++i) nt_issue(mine[i], ring + i * NT_STAGE, ring + WN_DESC_OFF + i * 16, ring + WN_BAR_OFF + i * 8);
-    if (WN_STAGES < n) upcoming = mine[WN_STAGES];
-  }
-  __syncwarp();
-  int st = 0; uint32_t phase = 0;
-  for (int k = 0; k < n; ++k) {
-    nt_wait(ring + WN_BAR_OFF + st * 8, phase);
-    const uint4 d = lds128(ring + WN_DESC_OFF + st * 16);
-    const uint32_t s = d.z;
-    const int nbytes = (int)(d.w & 0xFFFu);
-    const bool first_row = (d.w >> 30) & 1u;
-    const uint32_t body = ring + st * NT_STAGE + NT_HALO;
+  ring.start();
+  for (int k = 0; k < ring.n; ++k) {
+    const auto [src, s, nbytes, first_row, last_row, body] = ring.wait();
     uint32_t w[17];
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
       const uint4 v = lds128(body + lane * NT_CHUNK + q * 16);
       w[4 * q] = v.x; w[4 * q + 1] = v.y; w[4 * q + 2] = v.z; w[4 * q + 3] = v.w;
     }
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(w[16]) : "r"(body + lane * NT_CHUNK + NT_CHUNK));   // the 3 bytes after the chunk
+    w[16] = lds32(body + lane * NT_CHUNK + NT_CHUNK);             // the 3 bytes after the chunk
     __syncwarp();
-    if (lane == 0 && k + WN_STAGES < n) {
-      nt_issue(upcoming, ring + st * NT_STAGE, ring + WN_DESC_OFF + st * 16, ring + WN_BAR_OFF + st * 8);
-      if (k + WN_STAGES + 1 < n) upcoming = mine[k + WN_STAGES + 1];
-    }
-    if (++st == WN_STAGES) { st = 0; phase ^= 1u; }
+    ring.release(k);
 
-    const uint64_t src = (uint64_t)d.x | ((uint64_t)d.y << 32);
     const long long off = (long long)(src - (uint64_t)(uintptr_t)p.bytes) - p.starts[s] + (first_row ? 0 : NT_HALO);   // row in the sequence
     const long long woff = p.win_off[s], limit = (p.win_off[s + 1] - woff) * W;                      // bytes that have a window
     if (off >= limit) continue;                                                                     // same in every lane
@@ -237,12 +214,6 @@ __global__ void __launch_bounds__(WN_THREADS) window_dist_kernel(const uint32_t 
   if (lane == 0) td[win] = half + other;
 }
 
-uint32_t wn_revcomp(uint32_t x) {
-  uint32_t r = 0;
-  for (int i = 0; i < 4; ++i) { r = (r << 2) | ((x & 3u) ^ 3u); x >>= 2; }
-  return r;
-}
-
 }  // namespace
 
 extern "C" {
@@ -260,11 +231,8 @@ int ckm_window_stats(ckm_engine *e, const uint8_t *bytes, int64_t nbytes, const 
   }
   if (kernel_ms_out) *kernel_ms_out = 0.0f;
   if (win_off[0] != 0) { set_error("ckm_window_stats: win_off[0] must be 0"); return CKM_EINVAL; }
+  if (int rc = nt_check_layout("ckm_window_stats", "sequence", starts, lens, nseq, nbytes)) return rc;
   for (int32_t s = 0; s < nseq; ++s) {
-    if ((starts[s] & 63) || lens[s] < 0 || lens[s] > 0xFFFFFFFFll || starts[s] < 0 || (starts[s] + lens[s] + 63) / 64 * 64 > nbytes) {
-      set_error("ckm_window_stats: every sequence must start at a multiple of 64 bytes and lie, padded to 64, inside the buffer");
-      return CKM_EINVAL;
-    }
     const int64_t want = std::max<int64_t>(lens[s] - 1, 0) / window_size;
     if (win_off[s + 1] - win_off[s] != want) {
       std::snprintf(msg, sizeof msg, "ckm_window_stats: sequence %d has %lld windows in win_off, (length - 1) / window size is %lld",
@@ -278,24 +246,21 @@ int ckm_window_stats(ckm_engine *e, const uint8_t *bytes, int64_t nbytes, const 
   cudaSetDevice(e->device);
   PoolScope pool_scope(e);
   cudaStream_t st = e->stream;
-  DevBuf dbytes;
-  { int rc0 = dbytes.alloc((size_t)nbytes + 64); if (rc0) return rc0; }
-  std::vector<NtRow> rows;
-  nt_build_rows(dbytes.as<uint8_t>(), starts, lens, nseq, nbytes, rows);
-  const int64_t nrows = (int64_t)rows.size();
-  if (nrows > 0x7FFFFFFFll) { set_error("ckm_window_stats: too many bytes for one call"); return CKM_EINVAL; }
+  const int dyn_smem = WN_WARPS * WN_WARP_SMEM;
+  NtUpload u;
+  if (int rc = nt_upload(e, "ckm_window_stats", bytes, nbytes, starts, lens, nseq, (const void *)window_scan_kernel, WN_WARPS,
+                         WN_CTAS_PER_SM, dyn_smem, u))
+    return rc;
   std::vector<long long> seq_info((size_t)2 * nseq + 1);           // starts, then win_off
   for (int32_t s = 0; s < nseq; ++s) seq_info[s] = starts[s];
   for (int32_t s = 0; s <= nseq; ++s) seq_info[(size_t)nseq + s] = win_off[s];
-  DevBuf drows, dinfo, dacgt, dkm, dsig, dtd;
+  DevBuf dinfo, dacgt, dkm, dsig, dtd;
   int rc;
   const size_t km_bytes = bin_sig ? sizeof(uint32_t) * WN_COLS * (size_t)nwin : 0;
-  if ((rc = drows.alloc(sizeof(NtRow) * nrows)) || (rc = dinfo.alloc(sizeof(long long) * seq_info.size())) ||
+  if ((rc = dinfo.alloc(sizeof(long long) * seq_info.size())) ||
       (rc = dacgt.alloc(sizeof(int64_t) * 4 * (size_t)nwin)) ||
       (bin_sig && ((rc = dkm.alloc(km_bytes)) || (rc = dsig.alloc(sizeof(double) * WN_COLS)) || (rc = dtd.alloc(sizeof(double) * (size_t)nwin)))))
     return rc;
-  CKM_CUDA(cudaMemcpyAsync(dbytes.p, bytes, (size_t)nbytes, cudaMemcpyHostToDevice, st));
-  CKM_CUDA(cudaMemcpyAsync(drows.p, rows.data(), sizeof(NtRow) * nrows, cudaMemcpyHostToDevice, st));
   CKM_CUDA(cudaMemcpyAsync(dinfo.p, seq_info.data(), sizeof(long long) * seq_info.size(), cudaMemcpyHostToDevice, st));
   CKM_CUDA(cudaMemsetAsync(dacgt.p, 0, sizeof(int64_t) * 4 * (size_t)nwin, st));
   if (bin_sig) {
@@ -304,20 +269,16 @@ int ckm_window_stats(ckm_engine *e, const uint8_t *bytes, int64_t nbytes, const 
   }
   WinParams q;
   std::memset(&q, 0, sizeof(q));
-  q.bytes = dbytes.as<uint8_t>(); q.rows = drows.as<NtRow>(); q.nrows = nrows;
+  q.bytes = u.bytes.as<uint8_t>(); q.rows = u.rows.as<NtRow>(); q.nrows = u.nrows;
   q.starts = dinfo.as<long long>(); q.win_off = dinfo.as<long long>() + nseq; q.W = window_size;
   q.acgt = dacgt.as<unsigned long long>(); q.kmers = bin_sig ? dkm.as<uint32_t>() : nullptr;
   {
-    uint8_t col_of_canon[256]; int c = 0;                         // columns: canonical codes in ascending order
-    for (uint32_t x = 0; x < 256; ++x) if (x <= wn_revcomp(x)) col_of_canon[x] = (uint8_t)c++;
-    for (uint32_t x = 0; x < 256; ++x) q.col_of[x] = col_of_canon[std::min(x, wn_revcomp(x))];
+    uint8_t code[WN_COLS];                                        // a column and its code's reverse complement share it
+    for (int c = 0, n = km_col_codes(4, code); c < n; ++c) q.col_of[code[c]] = q.col_of[km_revcomp(code[c], 4)] = (uint8_t)c;
   }
-  const int grid = (int)std::min<int64_t>((int64_t)e->prop.multiProcessorCount * WN_CTAS_PER_SM, (nrows + WN_WARPS - 1) / WN_WARPS);
-  const int dyn_smem = WN_WARPS * WN_WARP_SMEM;
-  CKM_CUDA(cudaFuncSetAttribute(window_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn_smem));
   CKM_CUDA(cudaEventRecord(e->ev[0], st));
-  if (nrows > 0) {
-    window_scan_kernel<<<grid, WN_THREADS, dyn_smem, st>>>(q);
+  if (u.nrows > 0) {
+    window_scan_kernel<<<u.grid, WN_THREADS, dyn_smem, st>>>(q);
     CKM_CUDA(cudaGetLastError());
   }
   if (bin_sig) {
