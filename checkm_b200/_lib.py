@@ -83,7 +83,7 @@ class OutlierOut(C.Structure):
 SYMBOLS = ["ckm_init", "ckm_destroy", "ckm_last_error", "ckm_version", "ckm_device_name",
            "ckm_models_load", "ckm_models_count", "ckm_models_info", "ckm_models_find", "ckm_models_select",
            "ckm_models_write", "ckm_models_free", "ckm_digitize", "ckm_fasta_parse", "ckm_seqdb_create", "ckm_seqdb_free",
-           "ckm_search", "ckm_search_per_bin", "ckm_hits_free", "ckm_align", "ckm_last_stats", "ckm_msv_scores",
+           "ckm_search", "ckm_search_per_bin", "ckm_hits_free", "ckm_align", "ckm_align_groups", "ckm_aai_pairs", "ckm_last_stats", "ckm_msv_scores",
            "ckm_filter_scores", "ckm_viterbi_scores", "ckm_write_domtblout", "ckm_reduce", "ckm_genome_check", "ckm_free", "ckm_allgather_qa", "ckm_nccl_unique_id",
            "ckm_nccl_comm_init", "ckm_nccl_comm_destroy", "ckm_fasta_scan_nt", "ckm_scaffold_stats",
            "ckm_kmer_counts", "ckm_kmer_columns", "ckm_format_kmer_profiles", "ckm_merge_pairs", "ckm_format_merger_rows",
@@ -146,6 +146,8 @@ def lib():
     L.ckm_search.argtypes = [vp, vp, vp, i32, vp, dbl, dbl, C.POINTER(C.POINTER(Hit)), C.POINTER(i64)]
     L.ckm_search_per_bin.argtypes = [vp, vp, vp, vp, vp, dbl, dbl, C.POINTER(C.POINTER(Hit)), C.POINTER(i64)]
     L.ckm_align.argtypes = [vp, vp, i32, vp, vp, vp]
+    L.ckm_align_groups.argtypes = [vp, vp, vp, vp, i32, vp, vp, vp]
+    L.ckm_aai_pairs.argtypes = [vp, vp, vp, i64, vp, i64, vp, vp]
     L.ckm_hits_free.argtypes = [C.POINTER(Hit)]
     L.ckm_hits_free.restype = None
     L.ckm_last_stats.argtypes = [vp, C.POINTER(Stats)]

@@ -755,7 +755,12 @@ static int align_pass(ckm_engine *e, const SearchKnobs &k, const ckm_models *m, 
   return CKM_OK;
 }
 
-static int do_align(ckm_engine *e, const SearchKnobs &k, const ckm_models *m, int32_t model, const ckm_seqdb *db, int32_t *state_out, float *oasc_out) {
+// The group driver behind ckm_align and ckm_align_groups: the sequences of group g against model group_model[g], every group
+// in one align_pass (the envelope kernels take pairs of mixed models, as the search feeds them).  The groups' ranges of
+// sequences are disjoint (checked by the caller), so a sequence has one model.  The fallback searches the models of the
+// groups that have failed sequences in one call over `db`; a pair's domains do not depend on the other pairs of a search.
+static int do_align_groups(ckm_engine *e, const SearchKnobs &k, const ckm_models *m, const int32_t *group_model, const int64_t *group_seq_off,
+                           int32_t ngroups, const ckm_seqdb *db, int32_t *state_out, float *oasc_out) {
   std::memset(&e->stats, 0, sizeof(e->stats));
   const int nseq = db->nseq;
   for (int64_t i = 0; i < db->nres; ++i) state_out[i] = 0;
@@ -763,7 +768,7 @@ static int do_align(ckm_engine *e, const SearchKnobs &k, const ckm_models *m, in
   std::vector<PairWork> pairs;
   std::vector<Envelope> envs;
   int64_t rows = 0;
-  auto add = [&](int s, int i, int j) {
+  auto add = [&](int s, int model, int i, int j) {
     PairWork pw{};
     pw.seq = s; pw.model = model; pw.L = db->len[s]; pw.first_dom = (int32_t)pairs.size(); pw.ndom_slots = 1; pw.row_off = rows;
     rows += pw.L + 1;
@@ -771,35 +776,51 @@ static int do_align(ckm_engine *e, const SearchKnobs &k, const ckm_models *m, in
     en.pair = (int32_t)pairs.size(); en.i = i; en.j = j; en.null2_done = 1; en.slot = (int32_t)pairs.size();
     pairs.push_back(pw); envs.push_back(en);
   };
-  for (int s = 0; s < nseq; ++s) if (db->len[s] > 0) add(s, 1, db->len[s]);
+  for (int g = 0; g < ngroups; ++g)
+    for (int64_t s = group_seq_off[g]; s < group_seq_off[g + 1]; ++s) if (db->len[s] > 0) add((int)s, group_model[g], 1, db->len[s]);
   if (pairs.empty()) return CKM_OK;
   std::vector<int32_t> trace; std::vector<DomainOut> doms;
   int rc;
   if ((rc = align_pass(e, k, m, db, pairs, envs, rows, trace, doms))) return rc;
-  auto emit = [&](const std::vector<PairWork> &pp, const std::vector<DomainOut> &dd, const std::vector<int32_t> &tr, std::vector<int> *failed) {
+  auto emit = [&](const std::vector<PairWork> &pp, const std::vector<DomainOut> &dd, const std::vector<int32_t> &tr, std::vector<PairWork> *failed) {
     for (size_t pi = 0; pi < pp.size(); ++pi) {
       const PairWork &pw = pp[pi];
-      if (!dd[pi].ok) { if (failed) failed->push_back(pw.seq); continue; }
+      if (!dd[pi].ok) { if (failed) failed->push_back(pw); continue; }
       if (oasc_out) oasc_out[pw.seq] = dd[pi].oasc;
       int32_t *dst = state_out + (db->offsets[pw.seq] - db->offsets[0]);
       for (int i = 1; i <= pw.L; ++i) dst[i - 1] = tr[pw.row_off + i];
     }
   };
-  std::vector<int> failed;
+  std::vector<PairWork> failed;
   emit(pairs, doms, trace, &failed);
   if (failed.empty()) return CKM_OK;
   // the rare sequences one unihit envelope cannot hold: the envelope of the best domain the search pipeline defines
+  std::vector<int32_t> fmodels;
+  for (const PairWork &pw : failed) fmodels.push_back(pw.model);
+  std::sort(fmodels.begin(), fmodels.end());
+  fmodels.erase(std::unique(fmodels.begin(), fmodels.end()), fmodels.end());
   ckm_hit *hits = nullptr; int64_t nhits = 0;
-  if ((rc = do_search(e, k, m, &model, 1, nullptr, db, 1e300, 1e300, &hits, &nhits))) return rc;
-  std::vector<int> best(nseq, -1);
-  for (int64_t h = 0; h < nhits; ++h) { const int s = hits[h].seq; if (best[s] < 0 || hits[h].dom_score > hits[best[s]].dom_score) best[s] = (int)h; }
+  if ((rc = do_search(e, k, m, fmodels.data(), (int32_t)fmodels.size(), nullptr, db, 1e300, 1e300, &hits, &nhits))) return rc;
+  std::vector<int> model_of(nseq, -1), best(nseq, -1);
+  for (const PairWork &pw : failed) model_of[pw.seq] = pw.model;
+  for (int64_t h = 0; h < nhits; ++h) {
+    const int s = hits[h].seq;
+    if (hits[h].model != model_of[s]) continue;
+    if (best[s] < 0 || hits[h].dom_score > hits[best[s]].dom_score) best[s] = (int)h;
+  }
   pairs.clear(); envs.clear(); rows = 0;
-  for (int s : failed) if (best[s] >= 0) add(s, hits[best[s]].env_from, hits[best[s]].env_to);
+  for (const PairWork &pw : failed) if (best[pw.seq] >= 0) add(pw.seq, pw.model, hits[best[pw.seq]].env_from, hits[best[pw.seq]].env_to);
   std::free(hits);
   if (pairs.empty()) return CKM_OK;
   if ((rc = align_pass(e, k, m, db, pairs, envs, rows, trace, doms))) return rc;
   emit(pairs, doms, trace, nullptr);
   return CKM_OK;
+}
+
+static int checked_align(ckm_engine *e, const ckm_models *m, const int32_t *group_model, const int64_t *group_seq_off, int32_t ngroups,
+                         const ckm_seqdb *db, int32_t *state_out, float *oasc_out) {
+  cudaSetDevice(e->device);
+  return do_align_groups(e, read_knobs(true), m, group_model, group_seq_off, ngroups, db, state_out, oasc_out);
 }
 
 static int checked_search(ckm_engine *e, const ckm_models *m, const int32_t *model_idx, int32_t nmodels, const int64_t *bin_model_offsets,
@@ -825,8 +846,21 @@ int ckm_search_per_bin(ckm_engine *e, const ckm_models *m, const int32_t *model_
 int ckm_align(ckm_engine *e, const ckm_models *m, int32_t model, const ckm_seqdb *db, int32_t *state_out, float *oasc_out) {
   if (!e || !m || !db || !state_out) { set_error("ckm_align: bad argument"); return CKM_EINVAL; }
   if (model < 0 || model >= (int)m->models.size()) { set_error("ckm_align: model index out of range"); return CKM_EINVAL; }
-  cudaSetDevice(e->device);
-  return do_align(e, read_knobs(true), m, model, db, state_out, oasc_out);
+  const int64_t all[2] = {0, db->nseq};
+  return checked_align(e, m, &model, all, 1, db, state_out, oasc_out);
+}
+int ckm_align_groups(ckm_engine *e, const ckm_models *m, const int32_t *group_model, const int64_t *group_seq_off, int32_t ngroups,
+                     const ckm_seqdb *db, int32_t *state_out, float *oasc_out) {
+  if (!e || !m || !db || !state_out || ngroups < 0 || (ngroups > 0 && (!group_model || !group_seq_off))) {
+    set_error("ckm_align_groups: bad argument"); return CKM_EINVAL;
+  }
+  for (int32_t g = 0; g < ngroups; ++g) {
+    if (group_model[g] < 0 || group_model[g] >= (int)m->models.size()) { set_error("ckm_align_groups: model index out of range in group " + std::to_string(g)); return CKM_EINVAL; }
+    if (group_seq_off[g] < 0 || group_seq_off[g + 1] < group_seq_off[g] || group_seq_off[g + 1] > db->nseq) {
+      set_error("ckm_align_groups: group_seq_off must rise from >= 0 to <= nseq (group " + std::to_string(g) + ")"); return CKM_EINVAL;
+    }
+  }
+  return checked_align(e, m, group_model, group_seq_off, ngroups, db, state_out, oasc_out);
 }
 
 // domtblout writer: the 22 columns + description CheckM's HMMERParser.readHitsDOM splits (checkm/hmmer.py:184-200)

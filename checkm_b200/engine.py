@@ -195,6 +195,34 @@ class Engine:
         check(_lib.lib().ckm_align(self._h, models._h, int(model), db._h, state.ctypes.data, oasc.ctypes.data))
         return state, oasc
 
+    def align_groups(self, models, db, group_model, group_seq_off):
+        """`align` for many groups in one pass (ckm_align_groups): sequences group_seq_off[g]:group_seq_off[g + 1] of `db`
+        aligned to model group_model[g].  Returns the per-residue states and the per-sequence scores, as `align` does."""
+        gm = np.ascontiguousarray(group_model, dtype=np.int32)
+        go = np.ascontiguousarray(group_seq_off, dtype=np.int64)
+        if go.shape != (len(gm) + 1,):
+            raise ValueError("align_groups: group_seq_off must hold one offset per group and one more")
+        state = np.zeros(len(db.residues), dtype=np.int32)
+        oasc = np.zeros(db.nseq, dtype=np.float32)
+        check(_lib.lib().ckm_align_groups(self._h, models._h, gm.ctypes.data, go.ctypes.data, len(gm), db._h,
+                                          state.ctypes.data, oasc.ctypes.data))
+        return state, oasc
+
+    def aai_pairs(self, rows, row_off, pairs):
+        """Mismatches and compared length of every pair of masked alignment rows (ckm_aai_pairs).  rows: the rows' ASCII
+        bytes back to back, row r = rows[row_off[r]:row_off[r + 1]]; pairs: npairs x 2 row indices of rows of equal width.
+        Returns two int32 arrays of npairs values."""
+        rows = np.ascontiguousarray(np.frombuffer(rows, dtype=np.uint8) if not isinstance(rows, np.ndarray) else rows, dtype=np.uint8)
+        row_off = np.ascontiguousarray(row_off, dtype=np.int64)
+        pairs = np.ascontiguousarray(pairs, dtype=np.int32).reshape(-1, 2)
+        n = len(pairs)
+        mis = np.zeros(n, dtype=np.int32)
+        ln = np.zeros(n, dtype=np.int32)
+        check(_lib.lib().ckm_aai_pairs(self._h, rows.ctypes.data if rows.size else None, row_off.ctypes.data, len(row_off) - 1,
+                                       pairs.ctypes.data if n else None, n, mis.ctypes.data if n else None,
+                                       ln.ctypes.data if n else None))
+        return mis, ln
+
     def scaffold_stats(self, data, starts, lens):
         """Base counts and contigs of scaffolds laid out as `seqio.scan_nt_fasta` returns them (ckm_scaffold_stats).
         Returns stats (n x 8 int64: A C G T 'N' 'n' contigs contig-bases), the scaffold index and length of every contig

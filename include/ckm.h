@@ -164,6 +164,22 @@ void ckm_hits_free(ckm_hit *hits);
  * state_out[r] for residue r of the unpadded stream (ckm_seqdb_create offsets): k > 0 emitted by match state k, k < 0 by
  * insert state -k, 0 unaligned flank.  oasc_out[nseq] (optional): the optimal-accuracy score, 0 if no alignment exists. ---- */
 int  ckm_align(ckm_engine *e, const ckm_models *m, int32_t model, const ckm_seqdb *db, int32_t *state_out, float *oasc_out);
+/* the same for many groups in one pass (HmmerAligner: one group per marker, or per bin and multi-copy marker): sequences
+ * group_seq_off[g] .. group_seq_off[g+1]-1 of `db` aligned to model group_model[g].  group_seq_off (ngroups + 1) rises
+ * from >= 0 to <= nseq, so the groups are disjoint; sequences outside every group get state 0 and score 0.  Outputs as
+ * ckm_align's; each group's states and scores are those ckm_align returns for that group's sequences alone, including
+ * the fallback of a sequence one unihit envelope cannot hold (the envelope of its best domain against its group's model).
+ * ckm_align is this call with one group. */
+int  ckm_align_groups(ckm_engine *e, const ckm_models *m, const int32_t *group_model, const int64_t *group_seq_off,
+                      int32_t ngroups, const ckm_seqdb *db, int32_t *state_out, float *oasc_out);
+/* ---- amino-acid identity of masked alignment rows (checkm/aminoAcidIdentity.py:127-161), one warp per pair.
+ * rows: ASCII, '-' = gap; row r is rows[row_off[r] .. row_off[r+1]) (row_off: nrows + 1, non-decreasing, row_off[0] = 0).
+ * pairs: 2 * npairs row indices.  Per pair, over the columns [start, end) with start = the first column where neither row
+ * has a gap (the width if none) and end = 1 + the last column c >= 1 where neither has one (1 if none; the width if the
+ * width is < 2): mismatch_out = columns whose bytes differ, len_out = mismatches + equal columns that are not gaps.  The
+ * AAI is 1.0 - double(mismatches) / len, 0.0 when len is 0.  Rows of unequal width in a pair: CKM_EINVAL before any launch. */
+int  ckm_aai_pairs(ckm_engine *e, const uint8_t *rows, const int64_t *row_off, int64_t nrows, const int32_t *pairs,
+                   int64_t npairs, int32_t *mismatch_out, int32_t *len_out);
 int  ckm_last_stats(const ckm_engine *e, ckm_stats *out);
 
 /* stage-level entry points for parity tests (device arrays come back to host buffers the caller owns) */
