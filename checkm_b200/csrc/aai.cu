@@ -146,25 +146,21 @@ int ckm_aai_pairs(ckm_engine *e, const uint8_t *rows, const int64_t *row_off, in
   for (int64_t r = 0; r < nrows; ++r)
     if (width[(size_t)r]) std::memcpy(packed.data() + start[(size_t)r], rows + row_off[r], (size_t)width[(size_t)r]);
 
-  cudaSetDevice(e->device);
-  PoolScope pool_scope(e);
-  cudaStream_t st = e->stream;
+  const DeviceScope ws(e);
   DevBuf drows, dstart, dwidth, dpairs, dmis, dlen;
-  int rc;
-  if ((rc = drows.alloc(packed.size())) || (rc = dstart.alloc(sizeof(int64_t) * start.size())) ||
-      (rc = dwidth.alloc(sizeof(int32_t) * width.size())) || (rc = dpairs.alloc(sizeof(int2) * (size_t)npairs)) ||
-      (rc = dmis.alloc(sizeof(int32_t) * (size_t)npairs)) || (rc = dlen.alloc(sizeof(int32_t) * (size_t)npairs))) return rc;
-  CKM_CUDA(cudaMemcpyAsync(drows.p, packed.data(), packed.size(), cudaMemcpyHostToDevice, st));
-  CKM_CUDA(cudaMemcpyAsync(dstart.p, start.data(), sizeof(int64_t) * start.size(), cudaMemcpyHostToDevice, st));
-  CKM_CUDA(cudaMemcpyAsync(dwidth.p, width.data(), sizeof(int32_t) * width.size(), cudaMemcpyHostToDevice, st));
-  CKM_CUDA(cudaMemcpyAsync(dpairs.p, pairs, sizeof(int2) * (size_t)npairs, cudaMemcpyHostToDevice, st));
+  CKM_TRY(drows.put(packed.data(), packed.size(), ws.st));
+  CKM_TRY(dstart.put(start.data(), start.size(), ws.st));
+  CKM_TRY(dwidth.put(width.data(), width.size(), ws.st));
+  CKM_TRY(dpairs.put(reinterpret_cast<const int2 *>(pairs), (size_t)npairs, ws.st));
+  CKM_TRY(dmis.alloc(sizeof(int32_t) * (size_t)npairs));
+  CKM_TRY(dlen.alloc(sizeof(int32_t) * (size_t)npairs));
   const int64_t blocks = std::min<int64_t>((npairs + AAI_WARPS - 1) / AAI_WARPS, (int64_t)1 << 20);
-  aai_pairs_kernel<<<(unsigned)blocks, AAI_WARPS * 32, 0, st>>>(drows.as<uint8_t>(), dstart.as<int64_t>(), dwidth.as<int32_t>(),
-                                                               dpairs.as<int2>(), npairs, dmis.as<int32_t>(), dlen.as<int32_t>());
+  aai_pairs_kernel<<<(unsigned)blocks, AAI_WARPS * 32, 0, ws.st>>>(drows.as<uint8_t>(), dstart.as<int64_t>(), dwidth.as<int32_t>(),
+                                                                  dpairs.as<int2>(), npairs, dmis.as<int32_t>(), dlen.as<int32_t>());
   CKM_CUDA(cudaGetLastError());
-  CKM_CUDA(cudaMemcpyAsync(mismatch_out, dmis.p, sizeof(int32_t) * (size_t)npairs, cudaMemcpyDeviceToHost, st));
-  CKM_CUDA(cudaMemcpyAsync(len_out, dlen.p, sizeof(int32_t) * (size_t)npairs, cudaMemcpyDeviceToHost, st));
-  CKM_CUDA(cudaStreamSynchronize(st));
+  CKM_TRY(dmis.get(mismatch_out, (size_t)npairs, ws.st));
+  CKM_TRY(dlen.get(len_out, (size_t)npairs, ws.st));
+  CKM_TRY(stream_sync(ws.st));
   return CKM_OK;
 }
 

@@ -702,34 +702,32 @@ int inflate_batch(ckm_engine *e, const char *fn, const uint8_t *comp, int64_t co
   cudaStream_t st = e->stream;
   const int64_t total = uoff.back();
   DevBuf dcomp, dblk, duoff, dstat, dbad;
-  int rc;
-  if ((rc = dcomp.alloc((size_t)std::max<int64_t>(comp_len, 1))) || (rc = dblk.alloc(sizeof(ckm_bgzf_block) * (size_t)std::max<int64_t>(nblocks, 1))) ||
-      (rc = duoff.alloc(sizeof(int64_t) * (size_t)(nblocks + 1))) || (rc = dstat.alloc(sizeof(int) * (size_t)std::max<int64_t>(nblocks, 1))) ||
-      (rc = dbad.alloc(sizeof(unsigned long long))) || (rc = dout.alloc((size_t)total + 16)))
-    return rc;
-  if (comp_len) CKM_CUDA(cudaMemcpyAsync(dcomp.p, comp, (size_t)comp_len, cudaMemcpyHostToDevice, st));
-  if (nblocks) CKM_CUDA(cudaMemcpyAsync(dblk.p, blocks, sizeof(ckm_bgzf_block) * (size_t)nblocks, cudaMemcpyHostToDevice, st));
-  CKM_CUDA(cudaMemcpyAsync(duoff.p, uoff.data(), sizeof(int64_t) * (size_t)(nblocks + 1), cudaMemcpyHostToDevice, st));
-  CKM_CUDA(cudaMemsetAsync(dbad.p, 0xFF, sizeof(unsigned long long), st));
-  CKM_CUDA(cudaMemsetAsync(dout.as<uint8_t>() + total, 0, 16, st));
+  CKM_TRY(dcomp.put(comp, (size_t)comp_len, st));
+  CKM_TRY(dblk.put(blocks, (size_t)nblocks, st));
+  CKM_TRY(duoff.put(uoff.data(), uoff.size(), st));
+  CKM_TRY(dstat.alloc(sizeof(int) * (size_t)nblocks));
+  CKM_TRY(dbad.fill(sizeof(unsigned long long), 0xFF, st));
+  CKM_TRY(dout.alloc((size_t)total + 16));
+  CKM_TRY(set_bytes(dout.as<uint8_t>() + total, 0, 16, st));
   InflateParams p;
   p.comp = dcomp.as<uint8_t>(); p.comp_base = comp_base;
   p.blocks = dblk.as<ckm_bgzf_block>(); p.uoff = duoff.as<int64_t>(); p.nblocks = nblocks;
   p.out = dout.as<uint8_t>(); p.status = dstat.as<int>(); p.first_bad = dbad.as<unsigned long long>();
   std::memcpy(p.x2n, x2n_table(), sizeof(p.x2n));
-  CKM_CUDA(cudaEventRecord(e->ev[0], st));
+  CKM_TRY(ev_record(e, 0));
   if (nblocks) {
     bgzf_inflate_kernel<<<(unsigned)((nblocks + IW - 1) / IW), IW * 32, 0, st>>>(p);
     CKM_CUDA(cudaGetLastError());
   }
-  CKM_CUDA(cudaEventRecord(e->ev[1], st));
+  CKM_TRY(ev_record(e, 1));
   unsigned long long bad = 0;
-  CKM_CUDA(cudaMemcpyAsync(&bad, dbad.p, sizeof(bad), cudaMemcpyDeviceToHost, st));
-  CKM_CUDA(cudaStreamSynchronize(st));
-  CKM_CUDA(cudaEventElapsedTime(ms_out, e->ev[0], e->ev[1]));
+  CKM_TRY(dbad.get(&bad, 1, st));
+  CKM_TRY(stream_sync(st));
+  CKM_TRY(ev_elapsed(e, ms_out, 0, 1));
   if (bad != ~0ull) {
     int code = 0;
-    CKM_CUDA(cudaMemcpy(&code, dstat.as<int>() + bad, sizeof(int), cudaMemcpyDeviceToHost));
+    CKM_TRY(dstat.get(&code, 1, st, bad));
+    CKM_TRY(stream_sync(st));
     char msg[256];
     std::snprintf(msg, sizeof msg, "%s: BGZF block at file offset %lld: %s", fn, (long long)blocks[bad].coffset, inflate_msg(code));
     set_error(msg);
@@ -801,10 +799,8 @@ int walk_batch(const char *fn, ckm_engine *e, const uint8_t *comp, int64_t comp_
   std::vector<int64_t> uoff;
   int rc;
   if ((rc = check_batch(fn, comp_base, comp_len, blocks, nblocks, seg_start, seg_end, nseg, uoff))) return rc;
-  cudaSetDevice(e->device);
-  PoolScope pool_scope(e);
+  const DeviceScope ws(e);
   if ((rc = prepare())) return rc;
-  cudaStream_t st = e->stream;
   DevBuf dout, dseg, dcnt, derr;
   int64_t bad_block = -1;
   float ms_inflate = 0.0f;
@@ -814,32 +810,28 @@ int walk_batch(const char *fn, ckm_engine *e, const uint8_t *comp, int64_t comp_
   }
   if (kernel_ms_out) kernel_ms_out[0] = ms_inflate;
   const size_t ncnt = (size_t)n_ref * NCNT;
-  if ((rc = dseg.alloc(sizeof(int64_t) * 2 * (size_t)std::max<int64_t>(nseg, 1))) ||
-      (rc = dcnt.alloc(sizeof(int64_t) * std::max<size_t>(ncnt, 1))) || (rc = derr.alloc(sizeof(unsigned long long))))
-    return rc;
-  if (nseg) {
-    CKM_CUDA(cudaMemcpyAsync(dseg.p, seg_start, sizeof(int64_t) * (size_t)nseg, cudaMemcpyHostToDevice, st));
-    CKM_CUDA(cudaMemcpyAsync(dseg.as<int64_t>() + nseg, seg_end, sizeof(int64_t) * (size_t)nseg, cudaMemcpyHostToDevice, st));
-  }
-  if (ncnt) CKM_CUDA(cudaMemsetAsync(dcnt.p, 0, sizeof(int64_t) * ncnt, st));
-  CKM_CUDA(cudaMemsetAsync(derr.p, 0xFF, sizeof(unsigned long long), st));
+  CKM_TRY(dseg.alloc(sizeof(int64_t) * 2 * (size_t)nseg));
+  CKM_TRY(copy_in(dseg.as<int64_t>(), seg_start, (size_t)nseg, ws.st));
+  CKM_TRY(copy_in(dseg.as<int64_t>() + nseg, seg_end, (size_t)nseg, ws.st));
+  CKM_TRY(dcnt.fill(sizeof(int64_t) * ncnt, 0, ws.st));
+  CKM_TRY(derr.fill(sizeof(unsigned long long), 0xFF, ws.st));
   WalkParams q;
   q.data = dout.as<uint8_t>(); q.seg_start = dseg.as<int64_t>(); q.seg_end = dseg.as<int64_t>() + nseg; q.nseg = nseg;
   q.n_ref = n_ref; q.filter = *filter;
   q.counters = dcnt.as<unsigned long long>(); q.err = derr.as<unsigned long long>();
-  CKM_CUDA(cudaEventRecord(e->ev[0], st));
+  CKM_TRY(ev_record(e, 0));
   if (nseg) {
-    launch(q, (unsigned)((nseg + SCAN_THREADS - 1) / SCAN_THREADS), st);
+    launch(q, (unsigned)((nseg + SCAN_THREADS - 1) / SCAN_THREADS), ws.st);
     CKM_CUDA(cudaGetLastError());
   }
-  CKM_CUDA(cudaEventRecord(e->ev[1], st));
+  CKM_TRY(ev_record(e, 1));
   unsigned long long err = 0;
   std::vector<int64_t> cnt(ncnt);
-  CKM_CUDA(cudaMemcpyAsync(&err, derr.p, sizeof(err), cudaMemcpyDeviceToHost, st));
-  if (ncnt) CKM_CUDA(cudaMemcpyAsync(cnt.data(), dcnt.p, sizeof(int64_t) * ncnt, cudaMemcpyDeviceToHost, st));
-  CKM_CUDA(cudaStreamSynchronize(st));
+  CKM_TRY(derr.get(&err, 1, ws.st));
+  CKM_TRY(dcnt.get(cnt.data(), ncnt, ws.st));
+  CKM_TRY(stream_sync(ws.st));
   float ms_scan = 0.0f;
-  CKM_CUDA(cudaEventElapsedTime(&ms_scan, e->ev[0], e->ev[1]));
+  CKM_TRY(ev_elapsed(e, &ms_scan, 0, 1));
   if (kernel_ms_out) kernel_ms_out[1] = ms_scan;
   if (err != ~0ull) return scan_error(fn, err, blocks, nblocks, uoff, dout, err_offset_out);
   for (size_t k = 0; k < ncnt; ++k) counters[k] += cnt[k];
@@ -902,15 +894,14 @@ int ckm_bgzf_inflate(ckm_engine *e, const uint8_t *comp, int64_t comp_base, int6
   int rc;
   if ((rc = check_blocks("ckm_bgzf_inflate", comp_base, comp_len, blocks, nblocks, uoff))) return rc;
   if (uoff.back() > out_cap) { set_error("ckm_bgzf_inflate: output buffer smaller than the sum of ISIZE"); return CKM_ECAPACITY; }
-  cudaSetDevice(e->device);
-  PoolScope pool_scope(e);
+  const DeviceScope ws(e);
   DevBuf dout;
   float ms = 0.0f;
   if ((rc = inflate_batch(e, "ckm_bgzf_inflate", comp, comp_base, comp_len, blocks, nblocks, uoff, dout, bad_block_out, &ms)))
     return rc;
   if (kernel_ms_out) *kernel_ms_out = ms;
-  if (uoff.back()) CKM_CUDA(cudaMemcpy(out, dout.p, (size_t)uoff.back(), cudaMemcpyDeviceToHost));
-  return CKM_OK;
+  CKM_TRY(dout.get(out, (size_t)uoff.back(), ws.st));
+  return stream_sync(ws.st);
 }
 
 int ckm_bam_coverage(ckm_engine *e, const uint8_t *comp, int64_t comp_base, int64_t comp_len, const ckm_bgzf_block *blocks,
@@ -952,7 +943,7 @@ int ckm_bam_windows(ckm_engine *e, const uint8_t *comp, int64_t comp_base, int64
     size_t free_b = 0, total_b = 0;
     CKM_CUDA(cudaMemGetInfo(&free_b, &total_b));
     const double need = 8.0 * (double)nwin;
-    if (need > (double)free_b || dwin.alloc(sizeof(int64_t) * (size_t)std::max<int64_t>(nwin, 1))) {
+    if (need > (double)free_b || dwin.alloc(sizeof(int64_t) * (size_t)nwin)) {
       cudaGetLastError();
       if (need <= (double)free_b) CKM_CUDA(cudaMemGetInfo(&free_b, &total_b));
       // the smallest W whose window array fits in the free memory (sum of (len - 1) / W falls as W grows)
@@ -966,16 +957,13 @@ int ckm_bam_windows(ckm_engine *e, const uint8_t *comp, int64_t comp_base, int64
                     need / 1048576.0, (double)free_b / 1048576.0, (long long)lo_w);
       set_error(msg); return CKM_ENOMEM;
     }
-    int rc;
-    if ((rc = dlen.alloc(sizeof(int64_t) * (2 * (size_t)n_ref + 1))) || (rc = dtouch.alloc(2 * sizeof(unsigned long long))))
-      return rc;
     cudaStream_t st = e->stream;
-    if (nwin) CKM_CUDA(cudaMemsetAsync(dwin.p, 0, sizeof(int64_t) * (size_t)nwin, st));
+    CKM_TRY(set_bytes(dwin.p, 0, sizeof(int64_t) * (size_t)nwin, st));
     const unsigned long long touched0[2] = {~0ull, 0ull};
-    CKM_CUDA(cudaMemcpyAsync(dtouch.p, touched0, sizeof touched0, cudaMemcpyHostToDevice, st));
-    if (n_ref) CKM_CUDA(cudaMemcpyAsync(dlen.p, ref_len, sizeof(int64_t) * (size_t)n_ref, cudaMemcpyHostToDevice, st));
-    CKM_CUDA(cudaMemcpyAsync(dlen.as<int64_t>() + n_ref, win_off, sizeof(int64_t) * ((size_t)n_ref + 1), cudaMemcpyHostToDevice, st));
-    return CKM_OK;
+    CKM_TRY(dtouch.put(touched0, 2, st));
+    CKM_TRY(dlen.alloc(sizeof(int64_t) * (2 * (size_t)n_ref + 1)));
+    CKM_TRY(copy_in(dlen.as<int64_t>(), ref_len, (size_t)n_ref, st));
+    return copy_in(dlen.as<int64_t>() + n_ref, win_off, (size_t)n_ref + 1, st);
   };
   auto launch = [&](const WalkParams &w, unsigned grid, cudaStream_t st) {
     const WinParams q{w, dlen.as<int64_t>(), dlen.as<int64_t>() + n_ref, window_size, dwin.as<unsigned long long>(),
@@ -985,11 +973,13 @@ int ckm_bam_windows(ckm_engine *e, const uint8_t *comp, int64_t comp_base, int64
   // only the windows this batch wrote come back: a batch covers a run of references, not the whole array
   auto finish = [&]() -> int {
     unsigned long long touched[2];
-    CKM_CUDA(cudaMemcpy(touched, dtouch.p, sizeof touched, cudaMemcpyDeviceToHost));
+    CKM_TRY(dtouch.get(touched, 2, e->stream));
+    CKM_TRY(stream_sync(e->stream));
     if (touched[1] > touched[0]) {
       const size_t lo = (size_t)touched[0], n = (size_t)(touched[1] - touched[0]);
       std::vector<int64_t> w(n);
-      CKM_CUDA(cudaMemcpy(w.data(), dwin.as<int64_t>() + lo, sizeof(int64_t) * n, cudaMemcpyDeviceToHost));
+      CKM_TRY(dwin.get(w.data(), n, e->stream, lo));
+      CKM_TRY(stream_sync(e->stream));
       for (size_t k = 0; k < n; ++k) windows[lo + k] += w[k];
     }
     return CKM_OK;

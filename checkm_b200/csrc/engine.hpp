@@ -169,4 +169,5 @@ namespace ckm {
 void set_error(const std::string &msg);
 int  cuda_fail(cudaError_t e, const char *what);
 #define CKM_CUDA(call) do { cudaError_t _e = (call); if (_e != cudaSuccess) return ckm::cuda_fail(_e, #call); } while (0)
+#define CKM_TRY(expr) do { if (const int _rc = (expr)) return _rc; } while (0)
 }  // namespace ckm

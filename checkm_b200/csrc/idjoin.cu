@@ -201,32 +201,29 @@ int ckm_id_join(ckm_engine *e, const char *text, int64_t nbytes, int32_t nbins, 
   std::vector<int32_t> bin_of((size_t)std::max<int64_t>(nb, 1));
   { int64_t r = 0; for (int32_t b = 0; b < nbins; ++b) for (int64_t k = 0; k < bin_nrec[b]; ++k) bin_of[(size_t)r++] = b; }
 
-  cudaSetDevice(e->device);
-  PoolScope pool_scope(e);
-  cudaStream_t st = e->stream;
+  const DeviceScope ws(e);
   const unsigned long long cap = table_size(n), cap2 = table_size(nb);
-  const int64_t na = nasm, nbk = std::max<int64_t>(nb, 1);
+  const int64_t na = nasm;
   DevBuf dtext, dls, dbin, dis, dil, dh, dt, drep, dfa, dla, dfb, dt2, dl2, ds2, dflags, dlast, dkeep, dctr;
-  int rc;
-  if ((rc = dtext.alloc((size_t)nbytes)) || (rc = dls.alloc(sizeof(int64_t) * (n + 1))) || (rc = dbin.alloc(sizeof(int32_t) * nbk)) ||
-      (rc = dis.alloc(sizeof(int64_t) * n)) || (rc = dil.alloc(sizeof(int64_t) * n)) || (rc = dh.alloc(sizeof(unsigned long long) * n)) ||
-      (rc = dt.alloc(sizeof(unsigned long long) * cap)) || (rc = drep.alloc(sizeof(int32_t) * n)) ||
-      (rc = dfa.alloc(sizeof(int32_t) * n)) || (rc = dla.alloc(sizeof(int32_t) * n)) || (rc = dfb.alloc(sizeof(int32_t) * n)) ||
-      (rc = dt2.alloc(sizeof(unsigned long long) * cap2)) || (rc = dl2.alloc(sizeof(int32_t) * cap2)) ||
-      (rc = ds2.alloc(sizeof(int32_t) * nbk)) || (rc = dflags.alloc((size_t)std::max<int64_t>(na, 1))) ||
-      (rc = dlast.alloc(sizeof(int32_t) * std::max<int64_t>(na, 1))) || (rc = dkeep.alloc((size_t)nbk)) || (rc = dctr.alloc(64)))
-    return rc;
-  CKM_CUDA(cudaMemcpyAsync(dtext.p, text, (size_t)nbytes, cudaMemcpyHostToDevice, st));
-  CKM_CUDA(cudaMemcpyAsync(dls.p, line_start.data(), sizeof(int64_t) * (n + 1), cudaMemcpyHostToDevice, st));
-  if (nb) CKM_CUDA(cudaMemcpyAsync(dbin.p, bin_of.data(), sizeof(int32_t) * nb, cudaMemcpyHostToDevice, st));
-  CKM_CUDA(cudaMemsetAsync(dt.p, 0xFF, sizeof(unsigned long long) * cap, st));
-  CKM_CUDA(cudaMemsetAsync(dt2.p, 0xFF, sizeof(unsigned long long) * cap2, st));
-  CKM_CUDA(cudaMemsetAsync(dl2.p, 0xFF, sizeof(int32_t) * cap2, st));
-  CKM_CUDA(cudaMemsetAsync(dfa.p, 0x7F, sizeof(int32_t) * n, st));
-  CKM_CUDA(cudaMemsetAsync(dfb.p, 0x7F, sizeof(int32_t) * n, st));
-  CKM_CUDA(cudaMemsetAsync(dla.p, 0xFF, sizeof(int32_t) * n, st));
-  CKM_CUDA(cudaMemsetAsync(dctr.p, 0, 64, st));
-  CKM_CUDA(cudaMemsetAsync(dctr.p, 0xFF, 8, st));
+  CKM_TRY(dtext.put(text, (size_t)nbytes, ws.st));
+  CKM_TRY(dls.put(line_start.data(), (size_t)n + 1, ws.st));
+  CKM_TRY(dbin.put(bin_of.data(), (size_t)nb, ws.st));
+  CKM_TRY(dt.fill(sizeof(unsigned long long) * cap, 0xFF, ws.st));
+  CKM_TRY(dt2.fill(sizeof(unsigned long long) * cap2, 0xFF, ws.st));
+  CKM_TRY(dl2.fill(sizeof(int32_t) * cap2, 0xFF, ws.st));
+  CKM_TRY(dfa.fill(sizeof(int32_t) * n, 0x7F, ws.st));
+  CKM_TRY(dfb.fill(sizeof(int32_t) * n, 0x7F, ws.st));
+  CKM_TRY(dla.fill(sizeof(int32_t) * n, 0xFF, ws.st));
+  CKM_TRY(dctr.fill(64, 0, ws.st));
+  CKM_TRY(set_bytes(dctr.p, 0xFF, 8, ws.st));
+  CKM_TRY(dis.alloc(sizeof(int64_t) * n));
+  CKM_TRY(dil.alloc(sizeof(int64_t) * n));
+  CKM_TRY(dh.alloc(sizeof(unsigned long long) * n));
+  CKM_TRY(drep.alloc(sizeof(int32_t) * n));
+  CKM_TRY(ds2.alloc(sizeof(int32_t) * nb));
+  CKM_TRY(dflags.alloc((size_t)na));
+  CKM_TRY(dlast.alloc(sizeof(int32_t) * na));
+  CKM_TRY(dkeep.alloc((size_t)nb));
   IjParams p;
   p.text = dtext.as<uint8_t>(); p.line_start = dls.as<int64_t>(); p.bin_of = dbin.as<int32_t>(); p.n = n; p.nb = nb;
   p.id_start = dis.as<int64_t>(); p.id_len = dil.as<int64_t>(); p.hash = dh.as<unsigned long long>();
@@ -236,34 +233,32 @@ int ckm_id_join(ckm_engine *e, const char *text, int64_t nbytes, int32_t nbins, 
   p.asm_flags = dflags.as<uint8_t>(); p.asm_last = dlast.as<int32_t>(); p.bin_keep = dkeep.as<uint8_t>();
   p.counters = dctr.as<unsigned long long>();
   const unsigned grid = (unsigned)((n + IJ_THREADS - 1) / IJ_THREADS);
-  CKM_CUDA(cudaEventRecord(e->ev[0], st));
-  idjoin_find_kernel<<<grid, IJ_THREADS, 0, st>>>(p);
+  CKM_TRY(ev_record(e, 0));
+  idjoin_find_kernel<<<grid, IJ_THREADS, 0, ws.st>>>(p);
   CKM_CUDA(cudaGetLastError());
   unsigned long long ctr[2] = {0, 0};
-  CKM_CUDA(cudaMemcpyAsync(ctr, dctr.p, sizeof(ctr), cudaMemcpyDeviceToHost, st));
-  CKM_CUDA(cudaStreamSynchronize(st));
+  CKM_TRY(dctr.get(ctr, 2, ws.st));
+  CKM_TRY(stream_sync(ws.st));
   if (ctr[0] != IJ_EMPTY) {
     *bad_record_out = (int64_t)ctr[0];
     set_error("ckm_id_join: a header line without an id (record " + std::to_string((long long)ctr[0]) + ")");
     return CKM_EFORMAT;
   }
-  idjoin_insert_kernel<<<grid, IJ_THREADS, 0, st>>>(p);
+  idjoin_insert_kernel<<<grid, IJ_THREADS, 0, ws.st>>>(p);
   CKM_CUDA(cudaGetLastError());
-  idjoin_group_kernel<<<grid, IJ_THREADS, 0, st>>>(p);
+  idjoin_group_kernel<<<grid, IJ_THREADS, 0, ws.st>>>(p);
   CKM_CUDA(cudaGetLastError());
-  idjoin_emit_kernel<<<grid, IJ_THREADS, 0, st>>>(p);
+  idjoin_emit_kernel<<<grid, IJ_THREADS, 0, ws.st>>>(p);
   CKM_CUDA(cudaGetLastError());
-  CKM_CUDA(cudaEventRecord(e->ev[1], st));
-  CKM_CUDA(cudaMemcpyAsync(id_start_out, dis.p, sizeof(int64_t) * n, cudaMemcpyDeviceToHost, st));
-  CKM_CUDA(cudaMemcpyAsync(id_len_out, dil.p, sizeof(int64_t) * n, cudaMemcpyDeviceToHost, st));
-  if (na) {
-    CKM_CUDA(cudaMemcpyAsync(asm_flags_out, dflags.p, (size_t)na, cudaMemcpyDeviceToHost, st));
-    CKM_CUDA(cudaMemcpyAsync(asm_last_out, dlast.p, sizeof(int32_t) * na, cudaMemcpyDeviceToHost, st));
-  }
-  if (nb) CKM_CUDA(cudaMemcpyAsync(bin_keep_out, dkeep.p, (size_t)nb, cudaMemcpyDeviceToHost, st));
-  CKM_CUDA(cudaMemcpyAsync(ctr, dctr.p, sizeof(ctr), cudaMemcpyDeviceToHost, st));
-  CKM_CUDA(cudaStreamSynchronize(st));
-  if (kernel_ms_out) CKM_CUDA(cudaEventElapsedTime(kernel_ms_out, e->ev[0], e->ev[1]));
+  CKM_TRY(ev_record(e, 1));
+  CKM_TRY(dis.get(id_start_out, (size_t)n, ws.st));
+  CKM_TRY(dil.get(id_len_out, (size_t)n, ws.st));
+  CKM_TRY(dflags.get(asm_flags_out, (size_t)na, ws.st));
+  CKM_TRY(dlast.get(asm_last_out, (size_t)na, ws.st));
+  CKM_TRY(dkeep.get(bin_keep_out, (size_t)nb, ws.st));
+  CKM_TRY(dctr.get(ctr, 2, ws.st));
+  CKM_TRY(stream_sync(ws.st));
+  CKM_TRY(ev_elapsed(e, kernel_ms_out, 0, 1));
   *n_binned_ids_out = (int64_t)ctr[1];
   return CKM_OK;
 }

@@ -405,7 +405,7 @@ __global__ void __launch_bounds__(FWD_WARPS * 32) ensemble_kernel(EnsembleParams
 // The ensemble of all multi-domain regions as an asynchronous job on stream `st`: ensembles_launch enqueues the uploads,
 // the kernel and the downloads; ensembles_collect waits for them and hands back the envelopes of every region.
 struct EnsembleJob {
-  DevBuf b_regs, b_idx, b_off, b_scr, b_env, b_cnt, b_caps, b_eoff, b_need;       // workspaces from the engine's cache (the caller holds the PoolScope)
+  DevBuf b_regs, b_idx, b_off, b_scr, b_env, b_cnt, b_caps, b_eoff, b_need;       // workspaces from the engine's cache (the caller holds the DeviceScope)
   std::vector<int64_t> off, env_off;
   std::vector<Envelope> envs;
   std::vector<int32_t> cnt, need;
@@ -430,18 +430,15 @@ int ensembles_launch(ckm_engine *e, const ckm_models *m, DomdefParams &p, const 
     job->env_off[i] = nenv;
     nenv += caps[i].envelopes;
   }
-  int rc;
-  if ((rc = job->b_regs.alloc(sizeof(Region) * regs.size())) || (rc = job->b_idx.alloc(sizeof(int32_t) * nm)) || (rc = job->b_off.alloc(sizeof(int64_t) * nm)) ||
-      (rc = job->b_scr.alloc(sizeof(float) * (size_t)tot)) || (rc = job->b_env.alloc(sizeof(Envelope) * (size_t)nenv)) || (rc = job->b_cnt.alloc(sizeof(int32_t) * nm)) ||
-      (rc = job->b_caps.alloc(sizeof(EnsembleCaps) * nm)) || (rc = job->b_eoff.alloc(sizeof(int64_t) * nm)) || (rc = job->b_need.alloc(sizeof(int32_t) * 3 * nm))) return rc;
-  CKM_CUDA(cudaMemcpyAsync(job->b_regs.p, regs.data(), sizeof(Region) * regs.size(), cudaMemcpyHostToDevice, st));       // regs, multi_idx outlive the job (caller)
-  CKM_CUDA(cudaMemcpyAsync(job->b_idx.p, multi_idx.data(), sizeof(int32_t) * nm, cudaMemcpyHostToDevice, st));
-  CKM_CUDA(cudaMemcpyAsync(job->b_off.p, job->off.data(), sizeof(int64_t) * nm, cudaMemcpyHostToDevice, st));
-  CKM_CUDA(cudaMemcpyAsync(job->b_caps.p, job->caps.data(), sizeof(EnsembleCaps) * nm, cudaMemcpyHostToDevice, st));
-  CKM_CUDA(cudaMemcpyAsync(job->b_eoff.p, job->env_off.data(), sizeof(int64_t) * nm, cudaMemcpyHostToDevice, st));
-  CKM_CUDA(cudaMemsetAsync(job->b_cnt.p, 0, sizeof(int32_t) * nm, st));
-  CKM_CUDA(cudaMemsetAsync(job->b_need.p, 0, sizeof(int32_t) * 3 * nm, st));
-  CKM_CUDA(cudaMemsetAsync(job->b_env.p, 0, sizeof(Envelope) * (size_t)nenv, st));      // the kernel fills only the slots it uses; the whole block is copied back
+  CKM_TRY(job->b_regs.put(regs.data(), regs.size(), st));       // regs, multi_idx outlive the job (caller)
+  CKM_TRY(job->b_idx.put(multi_idx.data(), (size_t)nm, st));
+  CKM_TRY(job->b_off.put(job->off.data(), (size_t)nm, st));
+  CKM_TRY(job->b_scr.alloc(sizeof(float) * (size_t)tot));
+  CKM_TRY(job->b_env.fill(sizeof(Envelope) * (size_t)nenv, 0, st));      // the kernel fills only the slots it uses; the whole block is copied back
+  CKM_TRY(job->b_cnt.fill(sizeof(int32_t) * nm, 0, st));
+  CKM_TRY(job->b_caps.put(job->caps.data(), (size_t)nm, st));
+  CKM_TRY(job->b_eoff.put(job->env_off.data(), (size_t)nm, st));
+  CKM_TRY(job->b_need.fill(sizeof(int32_t) * 3 * nm, 0, st));
   EnsembleParams ep;
   ep.d = p; ep.regions = job->b_regs.as<Region>(); ep.multi_idx = job->b_idx.as<int32_t>(); ep.nmulti = nm;
   ep.scratch_off = job->b_off.as<int64_t>(); ep.scratch = job->b_scr.as<float>(); ep.env_out = job->b_env.as<Envelope>(); ep.env_count = job->b_cnt.as<int32_t>();
@@ -454,10 +451,9 @@ int ensembles_launch(ckm_engine *e, const ckm_models *m, DomdefParams &p, const 
   e->stats.kernel_launches++;
   job->envs.resize((size_t)nenv);
   job->cnt.resize(nm); job->need.resize((size_t)3 * nm);
-  CKM_CUDA(cudaMemcpyAsync(job->envs.data(), job->b_env.p, sizeof(Envelope) * job->envs.size(), cudaMemcpyDeviceToHost, st));
-  CKM_CUDA(cudaMemcpyAsync(job->cnt.data(), job->b_cnt.p, sizeof(int32_t) * nm, cudaMemcpyDeviceToHost, st));
-  CKM_CUDA(cudaMemcpyAsync(job->need.data(), job->b_need.p, sizeof(int32_t) * 3 * nm, cudaMemcpyDeviceToHost, st));
-  return CKM_OK;
+  CKM_TRY(job->b_env.get(job->envs.data(), job->envs.size(), st));
+  CKM_TRY(job->b_cnt.get(job->cnt.data(), (size_t)nm, st));
+  return job->b_need.get(job->need.data(), (size_t)3 * nm, st);
 }
 
 // out[i]: the envelopes of multi region i.  grow[i]: empty capacities (all zero) when the region fitted, else what it needs:

@@ -183,29 +183,25 @@ int ckm_kmer_counts(ckm_engine *e, const uint8_t *bytes, int64_t nbytes, const i
   if (int rc = nt_check_layout("ckm_kmer_counts", "sequence", starts, lens, nseq, nbytes)) return rc;
   const int ncols = km_cols(k);
   const size_t out_bytes = sizeof(uint32_t) * (size_t)ncols * (size_t)nseq;
-  cudaSetDevice(e->device);
-  PoolScope pool_scope(e);
-  cudaStream_t st = e->stream;
+  const DeviceScope ws(e);
   const int dyn_smem = KM_WARPS * KM_WARP_SMEM;
   void (*kern)(KmParams) = k == 1 ? kmer_kernel<1> : k == 2 ? kmer_kernel<2> : k == 3 ? kmer_kernel<3> : kmer_kernel<4>;
   NtUpload u;
-  if (int rc = nt_upload(e, "ckm_kmer_counts", bytes, nbytes, starts, lens, nseq, (const void *)kern, KM_WARPS, KM_CTAS_PER_SM, dyn_smem, u))
-    return rc;
+  CKM_TRY(nt_upload(e, "ckm_kmer_counts", bytes, nbytes, starts, lens, nseq, (const void *)kern, KM_WARPS, KM_CTAS_PER_SM, dyn_smem, u));
   if (u.nrows == 0) { std::memset(counts_out, 0, out_bytes); return CKM_OK; }
   DevBuf dcounts;
-  if (int rc = dcounts.alloc(out_bytes)) return rc;
-  CKM_CUDA(cudaMemsetAsync(dcounts.p, 0, out_bytes, st));
+  CKM_TRY(dcounts.fill(out_bytes, 0, ws.st));
   KmParams p;
   std::memset(&p, 0, sizeof(p));
   p.rows = u.rows.as<NtRow>(); p.nrows = u.nrows; p.counts = dcounts.as<uint32_t>();
   km_col_codes(k, p.col_code);
-  CKM_CUDA(cudaEventRecord(e->ev[0], st));
-  kern<<<u.grid, KM_THREADS, dyn_smem, st>>>(p);
+  CKM_TRY(ev_record(e, 0));
+  kern<<<u.grid, KM_THREADS, dyn_smem, ws.st>>>(p);
   CKM_CUDA(cudaGetLastError());
-  CKM_CUDA(cudaEventRecord(e->ev[1], st));
-  CKM_CUDA(cudaMemcpyAsync(counts_out, dcounts.p, out_bytes, cudaMemcpyDeviceToHost, st));
-  CKM_CUDA(cudaStreamSynchronize(st));
-  if (kernel_ms_out) CKM_CUDA(cudaEventElapsedTime(kernel_ms_out, e->ev[0], e->ev[1]));
+  CKM_TRY(ev_record(e, 1));
+  CKM_TRY(dcounts.get(counts_out, (size_t)ncols * (size_t)nseq, ws.st));
+  CKM_TRY(stream_sync(ws.st));
+  CKM_TRY(ev_elapsed(e, kernel_ms_out, 0, 1));
   return CKM_OK;
 }
 

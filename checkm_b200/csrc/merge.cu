@@ -214,40 +214,37 @@ int ckm_merge_pairs(ckm_engine *e, const int32_t *counts, int32_t nbins, int32_t
   q.Bp = q.nt * MG_TILE;
   q.min_delta_comp = min_delta_comp; q.max_delta_cont = max_delta_cont;
   q.min_merged_comp = min_merged_comp; q.max_merged_cont = max_merged_cont;
-  cudaSetDevice(e->device);
-  PoolScope pool_scope(e);
-  cudaStream_t st = e->stream;
+  const DeviceScope ws(e);
   const size_t nb = (size_t)nbins;
   DevBuf dcounts, dnmk, dbits, dp, ds, dcomp, dcont, dmask, drc, doff, dbad;
-  int rc;
-  if ((rc = dcounts.alloc(sizeof(int32_t) * nb * std::max(nmarkers, 1))) || (rc = dnmk.alloc(sizeof(int32_t) * nb)) ||
-      (rc = dbits.alloc(sizeof(uint32_t) * (size_t)q.W * q.Bp)) || (rc = dp.alloc(sizeof(int32_t) * nb)) ||
-      (rc = ds.alloc(sizeof(long long) * nb)) || (rc = dcomp.alloc(sizeof(double) * nb)) || (rc = dcont.alloc(sizeof(double) * nb)) ||
-      (rc = dmask.alloc(sizeof(unsigned long long) * nb * q.nt)) || (rc = drc.alloc(sizeof(unsigned long long) * nb)) ||
-      (rc = doff.alloc(sizeof(long long) * nb)) || (rc = dbad.alloc(sizeof(int))))
-    return rc;
+  CKM_TRY(dcounts.put(counts, nb * nmarkers, ws.st));
+  CKM_TRY(dnmk.put(n_markers, nb, ws.st));
+  CKM_TRY(dbits.fill(sizeof(uint32_t) * (size_t)q.W * q.Bp, 0, ws.st));
+  CKM_TRY(drc.fill(sizeof(unsigned long long) * nb, 0, ws.st));
+  CKM_TRY(dbad.fill(sizeof(int), 0, ws.st));
+  CKM_TRY(dp.alloc(sizeof(int32_t) * nb));
+  CKM_TRY(ds.alloc(sizeof(long long) * nb));
+  CKM_TRY(dcomp.alloc(sizeof(double) * nb));
+  CKM_TRY(dcont.alloc(sizeof(double) * nb));
+  CKM_TRY(dmask.alloc(sizeof(unsigned long long) * nb * q.nt));
+  CKM_TRY(doff.alloc(sizeof(long long) * nb));
   q.counts = dcounts.as<int32_t>(); q.nmk = dnmk.as<int32_t>(); q.bits = dbits.as<uint32_t>();
   q.p = dp.as<int32_t>(); q.s = ds.as<long long>(); q.comp = dcomp.as<double>(); q.cont = dcont.as<double>();
   q.mask = dmask.as<unsigned long long>(); q.rowcount = drc.as<unsigned long long>(); q.rowoff = doff.as<long long>();
   q.bad = dbad.as<int>();
-  if (nmarkers > 0) CKM_CUDA(cudaMemcpyAsync(dcounts.p, counts, sizeof(int32_t) * nb * nmarkers, cudaMemcpyHostToDevice, st));
-  CKM_CUDA(cudaMemcpyAsync(dnmk.p, n_markers, sizeof(int32_t) * nb, cudaMemcpyHostToDevice, st));
-  CKM_CUDA(cudaMemsetAsync(dbits.p, 0, sizeof(uint32_t) * (size_t)q.W * q.Bp, st));
-  CKM_CUDA(cudaMemsetAsync(drc.p, 0, sizeof(unsigned long long) * nb, st));
-  CKM_CUDA(cudaMemsetAsync(dbad.p, 0, sizeof(int), st));
-  CKM_CUDA(cudaEventRecord(e->ev[0], st));
-  merge_pack_kernel<<<(nbins + 7) / 8, 256, 0, st>>>(q);
+  CKM_TRY(ev_record(e, 0));
+  merge_pack_kernel<<<(nbins + 7) / 8, 256, 0, ws.st>>>(q);
   CKM_CUDA(cudaGetLastError());
-  merge_gram_kernel<<<dim3(q.nt, q.nt), MG_THREADS, 0, st>>>(q);
+  merge_gram_kernel<<<dim3(q.nt, q.nt), MG_THREADS, 0, ws.st>>>(q);
   CKM_CUDA(cudaGetLastError());
-  CKM_CUDA(cudaEventRecord(e->ev[1], st));
+  CKM_TRY(ev_record(e, 1));
   std::vector<unsigned long long> rowcount(nb);
   int bad = 0;
-  CKM_CUDA(cudaMemcpyAsync(rowcount.data(), drc.p, sizeof(unsigned long long) * nb, cudaMemcpyDeviceToHost, st));
-  CKM_CUDA(cudaMemcpyAsync(&bad, dbad.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CKM_CUDA(cudaStreamSynchronize(st));
+  CKM_TRY(drc.get(rowcount.data(), nb, ws.st));
+  CKM_TRY(dbad.get(&bad, 1, ws.st));
+  CKM_TRY(stream_sync(ws.st));
   float ms_gram = 0.0f;
-  CKM_CUDA(cudaEventElapsedTime(&ms_gram, e->ev[0], e->ev[1]));
+  CKM_TRY(ev_elapsed(e, &ms_gram, 0, 1));
   if (bad) {
     set_error("ckm_merge_pairs: copy numbers must be >= 0 and sum to less than 2^30 per bin");
     return CKM_EINVAL;
@@ -263,17 +260,17 @@ int ckm_merge_pairs(ckm_engine *e, const int32_t *counts, int32_t nbins, int32_t
   }
   if (total == 0) return CKM_OK;
   DevBuf dout;
-  if ((rc = dout.alloc(sizeof(int4) * (size_t)total))) return rc;
+  CKM_TRY(dout.alloc(sizeof(int4) * (size_t)total));
   q.out = dout.as<int4>();
-  CKM_CUDA(cudaMemcpyAsync(doff.p, rowoff.data(), sizeof(long long) * nb, cudaMemcpyHostToDevice, st));
-  CKM_CUDA(cudaEventRecord(e->ev[0], st));
-  merge_emit_kernel<<<(nbins + MG_EMIT_WARPS - 1) / MG_EMIT_WARPS, MG_EMIT_WARPS * 32, 0, st>>>(q);
+  CKM_TRY(copy_in(doff.as<long long>(), rowoff.data(), nb, ws.st));
+  CKM_TRY(ev_record(e, 0));
+  merge_emit_kernel<<<(nbins + MG_EMIT_WARPS - 1) / MG_EMIT_WARPS, MG_EMIT_WARPS * 32, 0, ws.st>>>(q);
   CKM_CUDA(cudaGetLastError());
-  CKM_CUDA(cudaEventRecord(e->ev[1], st));
-  CKM_CUDA(cudaMemcpyAsync(pairs_out, dout.p, sizeof(int4) * (size_t)total, cudaMemcpyDeviceToHost, st));
-  CKM_CUDA(cudaStreamSynchronize(st));
+  CKM_TRY(ev_record(e, 1));
+  CKM_TRY(dout.get(reinterpret_cast<int4 *>(pairs_out), (size_t)total, ws.st));
+  CKM_TRY(stream_sync(ws.st));
   float ms_emit = 0.0f;
-  CKM_CUDA(cudaEventElapsedTime(&ms_emit, e->ev[0], e->ev[1]));
+  CKM_TRY(ev_elapsed(e, &ms_emit, 0, 1));
   if (kernel_ms_out) *kernel_ms_out = ms_gram + ms_emit;
   return CKM_OK;
 }

@@ -163,18 +163,17 @@ struct NtUpload {
   int64_t nrows = 0;
   int grid = 0;                        // ctas_per_sm CTAs per SM, but no more warps than rows
 };
-// Copies the bytes and the row list to the device on the engine's stream (inside the caller's PoolScope) and lets `kernel`
+// Copies the bytes and the row list to the device on the engine's stream (inside the caller's DeviceScope) and lets `kernel`
 // take dyn_smem bytes of dynamic shared memory.  With no rows, nothing is copied and u.nrows is 0.
 inline int nt_upload(ckm_engine *e, const char *fn, const uint8_t *bytes, int64_t nbytes, const int64_t *starts, const int64_t *lens,
                      int32_t nseq, const void *kernel, int warps, int ctas_per_sm, int dyn_smem, NtUpload &u) {
-  if (int rc = u.bytes.alloc((size_t)nbytes + 64)) return rc;
+  CKM_TRY(u.bytes.alloc((size_t)nbytes + 64));
   nt_build_rows(u.bytes.as<uint8_t>(), starts, lens, nseq, nbytes, u.host_rows);
   u.nrows = (int64_t)u.host_rows.size();
   if (u.nrows == 0) return CKM_OK;
   if (u.nrows > 0x7FFFFFFFll) { set_error(std::string(fn) + ": too many bytes for one call"); return CKM_EINVAL; }
-  if (int rc = u.rows.alloc(sizeof(NtRow) * u.nrows)) return rc;
-  CKM_CUDA(cudaMemcpyAsync(u.bytes.p, bytes, (size_t)nbytes, cudaMemcpyHostToDevice, e->stream));
-  CKM_CUDA(cudaMemcpyAsync(u.rows.p, u.host_rows.data(), sizeof(NtRow) * u.nrows, cudaMemcpyHostToDevice, e->stream));
+  CKM_TRY(copy_in(u.bytes.as<uint8_t>(), bytes, (size_t)nbytes, e->stream));
+  CKM_TRY(u.rows.put(u.host_rows.data(), (size_t)u.nrows, e->stream));
   u.grid = (int)std::min<int64_t>((int64_t)e->prop.multiProcessorCount * ctas_per_sm, (u.nrows + warps - 1) / warps);
   CKM_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn_smem));
   return CKM_OK;

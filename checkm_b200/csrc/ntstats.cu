@@ -282,43 +282,38 @@ int ckm_scaffold_stats(ckm_engine *e, const uint8_t *bytes, int64_t nbytes, cons
   if (kernel_ms_out) *kernel_ms_out = 0.0f;
   if (nscaf == 0) return CKM_OK;
   if (int rc = nt_check_layout("ckm_scaffold_stats", "scaffold", starts, lens, nscaf, nbytes)) return rc;
-  cudaSetDevice(e->device);
-  PoolScope pool_scope(e);
-  cudaStream_t st = e->stream;
+  const DeviceScope ws(e);
   std::memset(stats_out, 0, sizeof(int64_t) * 8 * nscaf);
   const int dyn_smem = NT_WARPS * NT_WARP_SMEM;
   NtUpload u;
-  if (int rc = nt_upload(e, "ckm_scaffold_stats", bytes, nbytes, starts, lens, nscaf, (const void *)ntstats_kernel, NT_WARPS,
-                         NT_CTAS_PER_SM, dyn_smem, u))
-    return rc;
+  CKM_TRY(nt_upload(e, "ckm_scaffold_stats", bytes, nbytes, starts, lens, nscaf, (const void *)ntstats_kernel, NT_WARPS,
+                    NT_CTAS_PER_SM, dyn_smem, u));
   const int64_t nrows = u.nrows;
   if (nrows == 0) return CKM_OK;
   const int64_t nwarps = (int64_t)u.grid * NT_WARPS;
   const size_t npiece = (size_t)nscaf + nwarps;
   DevBuf dpiece, dstats, dcs, dcl, dctr;
-  int rc;
-  if ((rc = dpiece.alloc(sizeof(NtPiece) * npiece)) || (rc = dstats.alloc(sizeof(int64_t) * 8 * nscaf)) ||
-      (rc = dcs.alloc(sizeof(uint32_t) * (size_t)contig_cap)) || (rc = dcl.alloc(sizeof(uint32_t) * (size_t)contig_cap)) || (rc = dctr.alloc(64)))
-    return rc;
-  CKM_CUDA(cudaMemsetAsync(dpiece.p, 0, sizeof(NtPiece) * npiece, st));
-  CKM_CUDA(cudaMemsetAsync(dctr.p, 0, 64, st));
-  CKM_CUDA(cudaMemsetAsync(dstats.p, 0, sizeof(int64_t) * 8 * nscaf, st));
+  CKM_TRY(dpiece.fill(sizeof(NtPiece) * npiece, 0, ws.st));
+  CKM_TRY(dctr.fill(64, 0, ws.st));
+  CKM_TRY(dstats.fill(sizeof(int64_t) * 8 * nscaf, 0, ws.st));
+  CKM_TRY(dcs.alloc(sizeof(uint32_t) * (size_t)contig_cap));
+  CKM_TRY(dcl.alloc(sizeof(uint32_t) * (size_t)contig_cap));
   NtParams p;
   p.bytes = u.bytes.as<uint8_t>(); p.rows = u.rows.as<NtRow>(); p.nrows = nrows; p.piece = dpiece.as<NtPiece>();
   p.stats = dstats.as<unsigned long long>();
   p.contig_scaf = dcs.as<uint32_t>(); p.contig_len = dcl.as<uint32_t>();
   p.ncontigs = reinterpret_cast<unsigned long long *>(dctr.as<uint8_t>() + 8); p.cap = contig_cap;
-  CKM_CUDA(cudaEventRecord(e->ev[0], st));
-  ntstats_kernel<<<u.grid, NT_THREADS, dyn_smem, st>>>(p);
+  CKM_TRY(ev_record(e, 0));
+  ntstats_kernel<<<u.grid, NT_THREADS, dyn_smem, ws.st>>>(p);
   CKM_CUDA(cudaGetLastError());
-  CKM_CUDA(cudaEventRecord(e->ev[1], st));
+  CKM_TRY(ev_record(e, 1));
   unsigned long long n_dev = 0;
   std::vector<NtPiece> piece(npiece);
-  CKM_CUDA(cudaMemcpyAsync(&n_dev, p.ncontigs, sizeof(n_dev), cudaMemcpyDeviceToHost, st));
-  CKM_CUDA(cudaMemcpyAsync(stats_out, dstats.p, sizeof(int64_t) * 8 * nscaf, cudaMemcpyDeviceToHost, st));
-  CKM_CUDA(cudaMemcpyAsync(piece.data(), dpiece.p, sizeof(NtPiece) * npiece, cudaMemcpyDeviceToHost, st));
-  CKM_CUDA(cudaStreamSynchronize(st));
-  if (kernel_ms_out) CKM_CUDA(cudaEventElapsedTime(kernel_ms_out, e->ev[0], e->ev[1]));
+  CKM_TRY(copy_out(&n_dev, p.ncontigs, 1, ws.st));
+  CKM_TRY(dstats.get(stats_out, 8 * (size_t)nscaf, ws.st));
+  CKM_TRY(dpiece.get(piece.data(), npiece, ws.st));
+  CKM_TRY(stream_sync(ws.st));
+  CKM_TRY(ev_elapsed(e, kernel_ms_out, 0, 1));
   // join the open ends of the pieces, in list order: a contig runs from the tail of one piece through every piece without a
   // run end into the head of the next one of the same scaffold that has one
   std::vector<std::pair<uint32_t, uint32_t>> joined;
@@ -341,9 +336,9 @@ int ckm_scaffold_stats(ckm_engine *e, const uint8_t *bytes, int64_t nbytes, cons
   *ncontigs_out = n_found;
   if (n_found > contig_cap) { set_error("ckm_scaffold_stats: more contigs than the caller allowed for (the count is returned; call again)"); return CKM_ECAPACITY; }
   if (n_dev) {
-    CKM_CUDA(cudaMemcpyAsync(contig_scaffold_out, dcs.p, sizeof(uint32_t) * n_dev, cudaMemcpyDeviceToHost, st));
-    CKM_CUDA(cudaMemcpyAsync(contig_len_out, dcl.p, sizeof(uint32_t) * n_dev, cudaMemcpyDeviceToHost, st));
-    CKM_CUDA(cudaStreamSynchronize(st));
+    CKM_TRY(dcs.get(contig_scaffold_out, (size_t)n_dev, ws.st));
+    CKM_TRY(dcl.get(contig_len_out, (size_t)n_dev, ws.st));
+    CKM_TRY(stream_sync(ws.st));
   }
   for (size_t k = 0; k < joined.size(); ++k) {
     contig_scaffold_out[n_dev + k] = joined[k].first; contig_len_out[n_dev + k] = joined[k].second;

@@ -339,29 +339,30 @@ int ckm_outlier_scores(ckm_engine *e, const ckm_sigs *sigs, const ckm_outlier_in
     heap_off[b + 1] = heap_off[b] + ((2ll << depth[b]) - 1);
   }
   const long long nkeys = in->table_off[in->ntables];
-  cudaSetDevice(e->device);
-  PoolScope pool_scope(e);
-  cudaStream_t st = e->stream;
+  const DeviceScope ws(e);
   const size_t ns = (size_t)nseq, nb = (size_t)nbins;
   DevBuf dboff, dsbin, dlen, dacgt, dcod, drow, dbgc, dbcd, dtoff, dkey, dlo, dhi, dbsin, dbsig, dmeans, dseq, dtd, dmask, dhoff, ddepth, dheap;
-  int rc;
-  if ((rc = dboff.alloc(8 * (nb + 1))) || (rc = dsbin.alloc(4 * ns)) || (rc = dlen.alloc(8 * ns)) || (rc = dacgt.alloc(32 * ns)) ||
-      (rc = dcod.alloc(8 * ns)) || (rc = drow.alloc(8 * ns)) || (rc = dbgc.alloc(4 * nb)) || (rc = dbcd.alloc(4 * nb)) ||
-      (rc = dtoff.alloc(8 * ((size_t)in->ntables + 1))) || (rc = dkey.alloc(8 * (size_t)nkeys)) || (rc = dlo.alloc(8 * (size_t)nkeys)) ||
-      (rc = dhi.alloc(8 * (size_t)nkeys)) || (rc = dbsin.alloc(in->binsig_in ? 8 * nb * OL_COLS : 8)) ||
-      (rc = dbsig.alloc(8 * nb * OL_COLS)) || (rc = dmeans.alloc(8 * nb * 3)) || (rc = dseq.alloc(8 * ns * OL_SEQ_VALUES)) ||
-      (rc = dtd.alloc(8 * ns)) || (rc = dmask.alloc(ns)) || (rc = dhoff.alloc(8 * (nb + 1))) || (rc = ddepth.alloc(4 * nb)) ||
-      (rc = dheap.alloc(8 * (size_t)heap_off[nb])))
-    return rc;
-#define OL_UP(buf, src, bytes) CKM_CUDA(cudaMemcpyAsync((buf).p, (src), (bytes), cudaMemcpyHostToDevice, st))
-  OL_UP(dboff, in->bin_off, 8 * (nb + 1)); OL_UP(dsbin, seq_bin.data(), 4 * ns); OL_UP(dlen, in->len, 8 * ns);
-  OL_UP(dacgt, in->acgt, 32 * ns); OL_UP(dcod, in->coding, 8 * ns); OL_UP(drow, in->sig_row, 8 * ns);
-  OL_UP(dbgc, in->bin_gc_table, 4 * nb); OL_UP(dbcd, in->bin_cd_table, 4 * nb);
-  OL_UP(dtoff, in->table_off, 8 * ((size_t)in->ntables + 1)); OL_UP(dkey, in->table_key, 8 * (size_t)nkeys);
-  OL_UP(dlo, in->table_lo, 8 * (size_t)nkeys); OL_UP(dhi, in->table_hi, 8 * (size_t)nkeys);
-  if (in->binsig_in) OL_UP(dbsin, in->binsig_in, 8 * nb * OL_COLS);
-  OL_UP(dhoff, heap_off.data(), 8 * (nb + 1)); OL_UP(ddepth, depth.data(), 4 * nb);
-#undef OL_UP
+  CKM_TRY(dboff.put(in->bin_off, nb + 1, ws.st));
+  CKM_TRY(dsbin.put(seq_bin.data(), ns, ws.st));
+  CKM_TRY(dlen.put(in->len, ns, ws.st));
+  CKM_TRY(dacgt.put(in->acgt, 4 * ns, ws.st));
+  CKM_TRY(dcod.put(in->coding, ns, ws.st));
+  CKM_TRY(drow.put(in->sig_row, ns, ws.st));
+  CKM_TRY(dbgc.put(in->bin_gc_table, nb, ws.st));
+  CKM_TRY(dbcd.put(in->bin_cd_table, nb, ws.st));
+  CKM_TRY(dtoff.put(in->table_off, (size_t)in->ntables + 1, ws.st));
+  CKM_TRY(dkey.put(in->table_key, (size_t)nkeys, ws.st));
+  CKM_TRY(dlo.put(in->table_lo, (size_t)nkeys, ws.st));
+  CKM_TRY(dhi.put(in->table_hi, (size_t)nkeys, ws.st));
+  CKM_TRY(dbsin.put(in->binsig_in, in->binsig_in ? nb * OL_COLS : 0, ws.st));
+  CKM_TRY(dhoff.put(heap_off.data(), nb + 1, ws.st));
+  CKM_TRY(ddepth.put(depth.data(), nb, ws.st));
+  CKM_TRY(dbsig.alloc(8 * nb * OL_COLS));
+  CKM_TRY(dmeans.alloc(8 * nb * 3));
+  CKM_TRY(dseq.alloc(8 * ns * OL_SEQ_VALUES));
+  CKM_TRY(dtd.alloc(8 * ns));
+  CKM_TRY(dmask.alloc(ns));
+  CKM_TRY(dheap.alloc(8 * (size_t)heap_off[nb]));
   OutlierParams q;
   std::memset(&q, 0, sizeof(q));
   q.nseq = nseq; q.nbins = nbins;
@@ -372,22 +373,22 @@ int ckm_outlier_scores(ckm_engine *e, const ckm_sigs *sigs, const ckm_outlier_in
   q.binsig_in = in->binsig_in ? dbsin.as<double>() : nullptr;
   q.binsig = dbsig.as<double>(); q.means = dmeans.as<double>(); q.seq = dseq.as<double>(); q.td = dtd.as<double>();
   q.mask = dmask.as<unsigned char>(); q.heap_off = dhoff.as<long long>(); q.depth = ddepth.as<int>(); q.heap = dheap.as<double>();
-  CKM_CUDA(cudaEventRecord(e->ev[0], st));
-  outlier_bin_kernel<<<nbins, 160, 0, st>>>(q);
+  CKM_TRY(ev_record(e, 0));
+  outlier_bin_kernel<<<nbins, 160, 0, ws.st>>>(q);
   CKM_CUDA(cudaGetLastError());
-  CKM_CUDA(cudaEventRecord(e->ev[1], st));
-  outlier_seq_kernel<<<(unsigned)((nseq + 15) / 16), 256, 0, st>>>(q);
+  CKM_TRY(ev_record(e, 1));
+  outlier_seq_kernel<<<(unsigned)((nseq + 15) / 16), 256, 0, ws.st>>>(q);
   CKM_CUDA(cudaGetLastError());
-  CKM_CUDA(cudaEventRecord(e->ev[2], st));
-  outlier_mean_kernel<<<nbins, 256, 0, st>>>(q);
+  CKM_TRY(ev_record(e, 2));
+  outlier_mean_kernel<<<nbins, 256, 0, ws.st>>>(q);
   CKM_CUDA(cudaGetLastError());
-  CKM_CUDA(cudaEventRecord(e->ev[3], st));
-  CKM_CUDA(cudaMemcpyAsync(out->bin_means, dmeans.p, 8 * nb * 3, cudaMemcpyDeviceToHost, st));
-  if (out->bin_sig) CKM_CUDA(cudaMemcpyAsync(out->bin_sig, dbsig.p, 8 * nb * OL_COLS, cudaMemcpyDeviceToHost, st));
-  CKM_CUDA(cudaMemcpyAsync(out->seq_values, dseq.p, 8 * ns * OL_SEQ_VALUES, cudaMemcpyDeviceToHost, st));
-  CKM_CUDA(cudaMemcpyAsync(out->seq_mask, dmask.p, ns, cudaMemcpyDeviceToHost, st));
-  CKM_CUDA(cudaStreamSynchronize(st));
-  for (int k = 0; k < 3; ++k) CKM_CUDA(cudaEventElapsedTime(&out->kernel_ms[k], e->ev[k], e->ev[k + 1]));
+  CKM_TRY(ev_record(e, 3));
+  CKM_TRY(dmeans.get(out->bin_means, nb * 3, ws.st));
+  CKM_TRY(dbsig.get(out->bin_sig, out->bin_sig ? nb * OL_COLS : 0, ws.st));
+  CKM_TRY(dseq.get(out->seq_values, ns * OL_SEQ_VALUES, ws.st));
+  CKM_TRY(dmask.get(out->seq_mask, ns, ws.st));
+  CKM_TRY(stream_sync(ws.st));
+  for (int k = 0; k < 3; ++k) CKM_TRY(ev_elapsed(e, &out->kernel_ms[k], k, k + 1));
   return CKM_OK;
 }
 

@@ -12,6 +12,7 @@
 #include <cstring>
 #include <vector>
 #include "engine.hpp"
+#include "pool.hpp"
 
 namespace ckm {
 
@@ -332,24 +333,17 @@ extern "C" int ckm_genome_check(ckm_engine *e, int32_t nbins, const int64_t *bin
                                 const int32_t *marker_count, int32_t individual_markers, ckm_qa_row *rows_out) {
   if (!e || nbins < 0 || !bin_set_off || !set_marker_off || !rows_out) { set_error("ckm_genome_check: bad argument"); return CKM_EINVAL; }
   if (nbins == 0) return CKM_OK;
-  cudaSetDevice(e->device);
-  cudaStream_t st = e->stream;
+  const DeviceScope ws(e);
   const int64_t nsets = bin_set_off[nbins], nm = set_marker_off[nsets];
-  void *d_b = nullptr, *d_s = nullptr, *d_c = nullptr, *d_o = nullptr;
-  auto cleanup = [&]() { for (void *q : {d_b, d_s, d_c, d_o}) if (q) cudaFreeAsync(q, st); };       // stream-ordered pool: no device-wide synchronisation
-#define GCUDA(call) do { cudaError_t _e = (call); if (_e != cudaSuccess) { cleanup(); return cuda_fail(_e, #call); } } while (0)
-  GCUDA(cudaMallocAsync(&d_b, sizeof(int64_t) * (nbins + 1), st));
-  GCUDA(cudaMallocAsync(&d_s, sizeof(int64_t) * (size_t)(nsets + 1), st));
-  GCUDA(cudaMallocAsync(&d_c, sizeof(int32_t) * (size_t)std::max<int64_t>(nm, 1), st));
-  GCUDA(cudaMallocAsync(&d_o, sizeof(ckm_qa_row) * nbins, st));
-  GCUDA(cudaMemcpyAsync(d_b, bin_set_off, sizeof(int64_t) * (nbins + 1), cudaMemcpyHostToDevice, st));
-  GCUDA(cudaMemcpyAsync(d_s, set_marker_off, sizeof(int64_t) * (size_t)(nsets + 1), cudaMemcpyHostToDevice, st));
-  if (nm > 0) GCUDA(cudaMemcpyAsync(d_c, marker_count, sizeof(int32_t) * (size_t)nm, cudaMemcpyHostToDevice, st));
-  genome_check_kernel<<<(nbins + 127) / 128, 128, 0, st>>>(nbins, (const int64_t *)d_b, (const int64_t *)d_s, (const int32_t *)d_c, individual_markers, (ckm_qa_row *)d_o);
-  GCUDA(cudaGetLastError());
-  GCUDA(cudaMemcpyAsync(rows_out, d_o, sizeof(ckm_qa_row) * nbins, cudaMemcpyDeviceToHost, st));
-  GCUDA(cudaStreamSynchronize(st));
-  cleanup();
+  DevBuf d_b, d_s, d_c, d_o;
+  CKM_TRY(d_b.put(bin_set_off, (size_t)nbins + 1, ws.st));
+  CKM_TRY(d_s.put(set_marker_off, (size_t)nsets + 1, ws.st));
+  CKM_TRY(d_c.put(marker_count, (size_t)nm, ws.st));
+  CKM_TRY(d_o.alloc(sizeof(ckm_qa_row) * nbins));
+  genome_check_kernel<<<(nbins + 127) / 128, 128, 0, ws.st>>>(nbins, d_b.as<int64_t>(), d_s.as<int64_t>(), d_c.as<int32_t>(), individual_markers, d_o.as<ckm_qa_row>());
+  CKM_CUDA(cudaGetLastError());
+  CKM_TRY(d_o.get(rows_out, (size_t)nbins, ws.st));
+  CKM_TRY(stream_sync(ws.st));
   e->stats.kernel_launches++;
   return CKM_OK;
 }
@@ -359,8 +353,7 @@ extern "C" int ckm_reduce(ckm_engine *e, int32_t nmodels_in, int32_t nseq_in, in
                           const ckm_reduce_opts *opts, const ckm_reduce_meta *meta,
                           ckm_qa_row **qa_out, int32_t *nqa_out, ckm_marker_hit **mh_out, int64_t *nmh_out) {
   if (!e || nmodels_in < 0 || nseq_in < 0 || nbins_in < 1 || !opts || !meta || !qa_out || !nqa_out || !mh_out || !nmh_out || (nhits > 0 && !hits)) { set_error("ckm_reduce: bad argument"); return CKM_EINVAL; }
-  cudaSetDevice(e->device);
-  cudaStream_t st = e->stream;
+  const DeviceScope ws(e);
   const int nbins = nbins_in, nmodels = nmodels_in, nseq = nseq_in;
   *qa_out = nullptr; *mh_out = nullptr; *nqa_out = 0; *nmh_out = 0;
   // segments = maximal runs of equal (bin, model); rows of a bin must be contiguous and bins ascending (ckm_search order)
@@ -396,65 +389,63 @@ extern "C" int ckm_reduce(ckm_engine *e, int32_t nmodels_in, int32_t nseq_in, in
   const int64_t nsetm = (meta->set_marker_off && nsets > 0) ? meta->set_marker_off[nsets] : 0;
   std::vector<int64_t> zero_off(nbins + 1, 0), zero_set(1, 0);
 
-  std::vector<void *> frees;
-  auto dalloc = [&](size_t bytes) -> void * { void *p = nullptr; if (cudaMallocAsync(&p, std::max<size_t>(bytes, 16), st) != cudaSuccess) return nullptr; frees.push_back(p); return p; };
-  auto cleanup = [&]() { for (void *p : frees) cudaFreeAsync(p, st); };
-#define RCUDA(call) do { cudaError_t _e = (call); if (_e != cudaSuccess) { cleanup(); return cuda_fail(_e, #call); } } while (0)
-#define UP(dst, src, bytes) do { dst = (decltype(dst))dalloc(bytes); if (!dst) { cleanup(); set_error("ckm_reduce: out of device memory"); return CKM_ENOMEM; } if ((bytes) > 0) RCUDA(cudaMemcpyAsync((void *)dst, src, bytes, cudaMemcpyHostToDevice, st)); } while (0)
   RParams p;
   std::memset(&p, 0, sizeof(p));
   p.nhits = nhits; p.nseg = nseg; p.nbins = nbins; p.nmodels = nmodels; p.opts = *opts;
-  const size_t nh = (size_t)std::max<int64_t>(nhits, 1);
-  ckm_hit *d_hits; UP(d_hits, hits, sizeof(ckm_hit) * (size_t)nhits); p.hits = d_hits;
-  if (meta->row_scores != nullptr && nhits > 0) { double *d_rs; UP(d_rs, meta->row_scores, sizeof(double) * 2 * (size_t)nhits); p.row_scores = d_rs; }
-  p.rows = (RRow *)dalloc(sizeof(RRow) * nh); p.list = (int32_t *)dalloc(sizeof(int32_t) * nh); p.list_len = (int32_t *)dalloc(sizeof(int32_t) * std::max(nseg, 1));
-  p.filtered = (uint8_t *)dalloc(nh); p.first_app = (int64_t *)dalloc(sizeof(int64_t) * nh);
-  p.mh = (ckm_marker_hit *)dalloc(sizeof(ckm_marker_hit) * nh); p.mh_len = (int32_t *)dalloc(sizeof(int32_t) * std::max(nseg, 1));
-  p.qa = (ckm_qa_row *)dalloc(sizeof(ckm_qa_row) * nbins);
-  int32_t *d_overflow = (int32_t *)dalloc(sizeof(int32_t));
-  if (!p.rows || !p.list || !p.list_len || !p.filtered || !p.first_app || !p.mh || !p.mh_len || !p.qa || !d_overflow) { cleanup(); set_error("ckm_reduce: out of device memory"); return CKM_ENOMEM; }
-  RCUDA(cudaMemsetAsync(d_overflow, 0, sizeof(int32_t), st));
-  RCUDA(cudaMemsetAsync(p.mh_len, 0, sizeof(int32_t) * std::max(nseg, 1), st));
-  RModel *d_rm; UP(d_rm, rm.data(), sizeof(RModel) * rm.size()); p.models = d_rm;
-  int64_t *d_no; UP(d_no, nest_off, sizeof(int64_t) * (nmodels + 1)); p.nest_off = d_no;
-  int32_t *d_ni; UP(d_ni, meta->nest_idx, sizeof(int32_t) * (size_t)nnest); p.nest_idx = d_ni;
+  const size_t nh = (size_t)nhits;
   std::vector<int32_t> zero_seq(std::max(nseq, 1), 0);
-  int32_t *d_sc; UP(d_sc, meta->scaffold_id ? meta->scaffold_id : zero_seq.data(), sizeof(int32_t) * (size_t)nseq); p.scaffold_id = d_sc;
-  int32_t *d_on; UP(d_on, meta->orf_num ? meta->orf_num : zero_seq.data(), sizeof(int32_t) * (size_t)nseq); p.orf_num = d_on;
-  int32_t *d_nr; UP(d_nr, meta->name_rank ? meta->name_rank : zero_seq.data(), sizeof(int32_t) * (size_t)nseq); p.name_rank = d_nr;
-  int64_t *d_so; UP(d_so, seg_off.data(), sizeof(int64_t) * seg_off.size()); p.seg_off = d_so;
-  int32_t *d_sb; UP(d_sb, seg_bin.data(), sizeof(int32_t) * seg_bin.size()); p.seg_bin = d_sb;
-  int32_t *d_sm; UP(d_sm, seg_model.data(), sizeof(int32_t) * seg_model.size()); p.seg_model = d_sm;
-  int64_t *d_bro; UP(d_bro, bin_row_off.data(), sizeof(int64_t) * bin_row_off.size()); p.bin_row_off = d_bro;
-  int64_t *d_bso; UP(d_bso, bin_seg_off.data(), sizeof(int64_t) * bin_seg_off.size()); p.bin_seg_off = d_bso;
-  int64_t *d_bs; UP(d_bs, meta->bin_set_off ? meta->bin_set_off : zero_off.data(), sizeof(int64_t) * (nbins + 1)); p.bin_set_off = d_bs;
-  int64_t *d_smo; UP(d_smo, (meta->set_marker_off && nsets > 0) ? meta->set_marker_off : zero_set.data(), sizeof(int64_t) * (size_t)(nsets + 1)); p.set_marker_off = d_smo;
-  int32_t *d_smi; UP(d_smi, meta->set_marker_idx, sizeof(int32_t) * (size_t)nsetm); p.set_marker_idx = d_smi;
-  int32_t *d_sof; UP(d_sof, seg_of.data(), sizeof(int32_t) * seg_of.size()); p.seg_of_bin_model = d_sof;
+  DevBuf d_hits, d_rs, d_rows, d_list, d_list_len, d_filtered, d_first_app, d_mh, d_mh_len, d_qa, d_overflow, d_rm, d_no, d_ni, d_sc, d_on,
+         d_nr, d_so, d_sb, d_sm, d_bro, d_bso, d_bs, d_smo, d_smi, d_sof;
+  CKM_TRY(d_hits.put(hits, nh, ws.st)); p.hits = d_hits.as<ckm_hit>();
+  if (meta->row_scores != nullptr && nhits > 0) { CKM_TRY(d_rs.put(meta->row_scores, 2 * nh, ws.st)); p.row_scores = d_rs.as<double>(); }
+  CKM_TRY(d_rows.alloc(sizeof(RRow) * nh)); p.rows = d_rows.as<RRow>();
+  CKM_TRY(d_list.alloc(sizeof(int32_t) * nh)); p.list = d_list.as<int32_t>();
+  CKM_TRY(d_list_len.alloc(sizeof(int32_t) * nseg)); p.list_len = d_list_len.as<int32_t>();
+  CKM_TRY(d_filtered.alloc(nh)); p.filtered = d_filtered.as<uint8_t>();
+  CKM_TRY(d_first_app.alloc(sizeof(int64_t) * nh)); p.first_app = d_first_app.as<int64_t>();
+  CKM_TRY(d_mh.alloc(sizeof(ckm_marker_hit) * nh)); p.mh = d_mh.as<ckm_marker_hit>();
+  CKM_TRY(d_mh_len.fill(sizeof(int32_t) * nseg, 0, ws.st)); p.mh_len = d_mh_len.as<int32_t>();
+  CKM_TRY(d_qa.alloc(sizeof(ckm_qa_row) * nbins)); p.qa = d_qa.as<ckm_qa_row>();
+  CKM_TRY(d_overflow.fill(sizeof(int32_t), 0, ws.st));
+  CKM_TRY(d_rm.put(rm.data(), rm.size(), ws.st)); p.models = d_rm.as<RModel>();
+  CKM_TRY(d_no.put(nest_off, (size_t)nmodels + 1, ws.st)); p.nest_off = d_no.as<int64_t>();
+  CKM_TRY(d_ni.put(meta->nest_idx, (size_t)nnest, ws.st)); p.nest_idx = d_ni.as<int32_t>();
+  CKM_TRY(d_sc.put(meta->scaffold_id ? meta->scaffold_id : zero_seq.data(), (size_t)nseq, ws.st)); p.scaffold_id = d_sc.as<int32_t>();
+  CKM_TRY(d_on.put(meta->orf_num ? meta->orf_num : zero_seq.data(), (size_t)nseq, ws.st)); p.orf_num = d_on.as<int32_t>();
+  CKM_TRY(d_nr.put(meta->name_rank ? meta->name_rank : zero_seq.data(), (size_t)nseq, ws.st)); p.name_rank = d_nr.as<int32_t>();
+  CKM_TRY(d_so.put(seg_off.data(), seg_off.size(), ws.st)); p.seg_off = d_so.as<int64_t>();
+  CKM_TRY(d_sb.put(seg_bin.data(), seg_bin.size(), ws.st)); p.seg_bin = d_sb.as<int32_t>();
+  CKM_TRY(d_sm.put(seg_model.data(), seg_model.size(), ws.st)); p.seg_model = d_sm.as<int32_t>();
+  CKM_TRY(d_bro.put(bin_row_off.data(), bin_row_off.size(), ws.st)); p.bin_row_off = d_bro.as<int64_t>();
+  CKM_TRY(d_bso.put(bin_seg_off.data(), bin_seg_off.size(), ws.st)); p.bin_seg_off = d_bso.as<int64_t>();
+  CKM_TRY(d_bs.put(meta->bin_set_off ? meta->bin_set_off : zero_off.data(), (size_t)nbins + 1, ws.st)); p.bin_set_off = d_bs.as<int64_t>();
+  CKM_TRY(d_smo.put((meta->set_marker_off && nsets > 0) ? meta->set_marker_off : zero_set.data(), (size_t)nsets + 1, ws.st));
+  p.set_marker_off = d_smo.as<int64_t>();
+  CKM_TRY(d_smi.put(meta->set_marker_idx, (size_t)nsetm, ws.st)); p.set_marker_idx = d_smi.as<int32_t>();
+  CKM_TRY(d_sof.put(seg_of.data(), seg_of.size(), ws.st)); p.seg_of_bin_model = d_sof.as<int32_t>();
 
   const int T = 128;
   if (nhits > 0) {
-    r0_round_rows<<<(int)std::min<int64_t>((nhits + T - 1) / T, 4096), T, 0, st>>>(p);
-    r1_add_hits<<<(nseg + T - 1) / T, T, 0, st>>>(p);
-    r2_clan_filter<<<(nseg + 31) / 32, 32, 0, st>>>(p, d_overflow);
-    r3_adjacent<<<(nseg + T - 1) / T, T, 0, st>>>(p);
+    r0_round_rows<<<(int)std::min<int64_t>((nhits + T - 1) / T, 4096), T, 0, ws.st>>>(p);
+    r1_add_hits<<<(nseg + T - 1) / T, T, 0, ws.st>>>(p);
+    r2_clan_filter<<<(nseg + 31) / 32, 32, 0, ws.st>>>(p, d_overflow.as<int32_t>());
+    r3_adjacent<<<(nseg + T - 1) / T, T, 0, ws.st>>>(p);
   }
-  r4_counts<<<(nbins + T - 1) / T, T, 0, st>>>(p);
-  RCUDA(cudaGetLastError());
+  r4_counts<<<(nbins + T - 1) / T, T, 0, ws.st>>>(p);
+  CKM_CUDA(cudaGetLastError());
   e->stats.kernel_launches += 5;
-  std::vector<ckm_marker_hit> mh((size_t)nhits);
-  std::vector<int32_t> mh_len(std::max(nseg, 1), 0);
-  ckm_qa_row *qa = (ckm_qa_row *)std::malloc(sizeof(ckm_qa_row) * std::max(nbins, 1));
+  std::vector<ckm_marker_hit> mh(nh);
+  std::vector<int32_t> mh_len(nseg);
+  std::vector<ckm_qa_row> qa_rows(nbins);
   int32_t overflow = 0;
-  if (nhits > 0) {
-    RCUDA(cudaMemcpyAsync(mh.data(), p.mh, sizeof(ckm_marker_hit) * (size_t)nhits, cudaMemcpyDeviceToHost, st));
-    RCUDA(cudaMemcpyAsync(mh_len.data(), p.mh_len, sizeof(int32_t) * nseg, cudaMemcpyDeviceToHost, st));
-  }
-  RCUDA(cudaMemcpyAsync(qa, p.qa, sizeof(ckm_qa_row) * nbins, cudaMemcpyDeviceToHost, st));
-  RCUDA(cudaMemcpyAsync(&overflow, d_overflow, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-  RCUDA(cudaStreamSynchronize(st));
-  cleanup();
-  if (overflow) { std::free(qa); set_error("ckm_reduce: more than 384 Pfam hits on one ORF"); return CKM_ECAPACITY; }
+  CKM_TRY(d_mh.get(mh.data(), nh, ws.st));
+  CKM_TRY(d_mh_len.get(mh_len.data(), (size_t)nseg, ws.st));
+  CKM_TRY(d_qa.get(qa_rows.data(), (size_t)nbins, ws.st));
+  CKM_TRY(d_overflow.get(&overflow, 1, ws.st));
+  CKM_TRY(stream_sync(ws.st));
+  if (overflow) { set_error("ckm_reduce: more than 384 Pfam hits on one ORF"); return CKM_ECAPACITY; }
+  ckm_qa_row *qa = (ckm_qa_row *)std::malloc(sizeof(ckm_qa_row) * nbins);
+  std::memcpy(qa, qa_rows.data(), sizeof(ckm_qa_row) * nbins);
   // compact the per-segment lists
   int64_t total = 0;
   for (int s = 0; s < nseg; ++s) total += mh_len[s];

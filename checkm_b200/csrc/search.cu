@@ -153,7 +153,7 @@ static void fill_filter_stats(ckm_engine *e, int64_t n_pairs, const int32_t *ctr
   s.n_ssv_cand = (int64_t)ctr[CTR_CAND] + ctr[CTR_SSVRES]; s.n_msv_exact = ctr[CTR_CAND]; s.n_past_msv = ctr[CTR_MSV]; s.n_past_bias = ctr[CTR_BIAS];
   s.n_past_vit = ctr[CTR_VIT]; s.n_past_fwd = ctr[CTR_FWD]; s.n_vit_redo = ctr[CTR_VREDO];
   float *ms[] = {&s.ms_ssv, &s.ms_msv, &s.ms_bias, &s.ms_vit, &s.ms_fwd};
-  for (int i = 0; i < stages; ++i) cudaEventElapsedTime(ms[i], e->ev[EV_SSV + i], e->ev[EV_SSV + i + 1]);
+  for (int i = 0; i < stages; ++i) ev_elapsed(e, ms[i], EV_SSV + i, EV_SSV + i + 1);
 }
 static std::vector<float> &logsum_table() {
   static std::vector<float> t = [] {
@@ -180,9 +180,7 @@ static int build_masks(const ckm_models *m, const ckm_seqdb *db, const int32_t *
     if (all) for (int i = 0; i < ndb; ++i) if (slot_of_model[i] < 0) all = false;
   }
   am.all_active = all;
-  int rc;
-  if ((rc = am.model_slot.alloc(sizeof(int32_t) * ndb))) return rc;
-  CKM_CUDA(cudaMemcpyAsync(am.model_slot.p, slot_of_model.data(), sizeof(int32_t) * ndb, cudaMemcpyHostToDevice, st));
+  CKM_TRY(am.model_slot.put(slot_of_model.data(), (size_t)ndb, st));
   if (all) return CKM_OK;
   std::vector<uint8_t> ma((size_t)nbins * ndb, 0), ta((size_t)nbins * ntiles, 0);
   for (int b = 0; b < nbins; ++b) {
@@ -204,12 +202,9 @@ static int build_masks(const ckm_models *m, const ckm_seqdb *db, const int32_t *
     }
     // a chained model is addressed through its first tile
   }
-  if ((rc = am.model_active.alloc(ma.size()))) return rc;
-  if ((rc = am.tile_active.alloc(ta.size()))) return rc;
-  CKM_CUDA(cudaMemcpyAsync(am.model_active.p, ma.data(), ma.size(), cudaMemcpyHostToDevice, st));
-  CKM_CUDA(cudaMemcpyAsync(am.tile_active.p, ta.data(), ta.size(), cudaMemcpyHostToDevice, st));
-  CKM_CUDA(cudaStreamSynchronize(st));     // host vectors go out of scope
-  return CKM_OK;
+  CKM_TRY(am.model_active.put(ma.data(), ma.size(), st));
+  CKM_TRY(am.tile_active.put(ta.data(), ta.size(), st));
+  return stream_sync(st);     // host vectors go out of scope
 }
 // Stage 1: SSV pre-filter over all pairs -> candidate list; exact MSV on the candidates -> pass list.
 struct Stage1 {
@@ -235,27 +230,25 @@ static int run_stage1(ckm_engine *e, const SearchKnobs &k, const ckm_models *m, 
   const int64_t n_bypass = (int64_t)m->ssv_bypass.size() * db->nseq;          // models without SSV tiles: every pair is a candidate
   s1.cand_cap = (int32_t)std::min<int64_t>(QUEUE_MAX, (int64_t)s1.cand_cap + n_bypass);
   s1.pass_cap = queue_cap(n_pairs, 12, attempt);
-  if ((rc = s1.cand.alloc(sizeof(int2) * (size_t)s1.cand_cap))) return rc;
-  if ((rc = s1.pass.alloc(sizeof(Candidate) * (size_t)s1.pass_cap))) return rc;
-  if ((rc = s1.cells.alloc(sizeof(unsigned long long)))) return rc;
-  CKM_CUDA(cudaMemsetAsync(e->d_counters, 0, CTR_N * sizeof(int32_t), st));
-  CKM_CUDA(cudaMemsetAsync(s1.cells.p, 0, sizeof(unsigned long long), st));
+  CKM_TRY(s1.cand.alloc(sizeof(int2) * (size_t)s1.cand_cap));
+  CKM_TRY(s1.pass.alloc(sizeof(Candidate) * (size_t)s1.pass_cap));
+  CKM_TRY(set_bytes(e->d_counters, 0, CTR_N * sizeof(int32_t), st));
+  CKM_TRY(s1.cells.fill(sizeof(unsigned long long), 0, st));
   const int nsm = e->prop.multiProcessorCount;
   bool need_bnd = false;
   for (int nt : m->chain_ntiles) need_bnd |= (nt > 1);
   const int64_t bnd_stride = ((int64_t)db->maxL + 31) / 16 * 16;
-  if (need_bnd) { if ((rc = s1.bnd.alloc((size_t)nsm * SSV_WARPS_HOST * 2 * bnd_stride * sizeof(int16_t)))) return rc; }
+  if (need_bnd) CKM_TRY(s1.bnd.alloc((size_t)nsm * SSV_WARPS_HOST * 2 * bnd_stride * sizeof(int16_t)));
   // group lists per J
   std::vector<int32_t> gl[4];
   for (size_t g = 0; g < m->groups.size(); ++g) gl[m->groups[g].J == 4 ? 0 : (m->groups[g].J == 8 ? 1 : (m->groups[g].J == 16 ? 2 : 3))].push_back((int32_t)g);
   std::vector<int32_t> flat;
   size_t goff[4];
   for (int c = 0; c < 4; ++c) { goff[c] = flat.size(); flat.insert(flat.end(), gl[c].begin(), gl[c].end()); }
-  if ((rc = s1.glist.alloc(sizeof(int32_t) * std::max<size_t>(flat.size(), 1)))) return rc;
-  if (!flat.empty()) CKM_CUDA(cudaMemcpyAsync(s1.glist.p, flat.data(), sizeof(int32_t) * flat.size(), cudaMemcpyHostToDevice, st));
-  CKM_CUDA(cudaStreamSynchronize(st));     // `flat` is read by the copy above
+  CKM_TRY(s1.glist.put(flat.data(), flat.size(), st));
+  CKM_TRY(stream_sync(st));     // `flat` is read by the copy above
 
-  CKM_CUDA(cudaEventRecord(e->ev[EV_SSV], st));
+  CKM_TRY(ev_record(e, EV_SSV));
   SsvParams sp{};
   sp.res = db->d_res; sp.off = db->d_off; sp.len = db->d_len; sp.bin = db->d_bin;
   sp.msvB = db->d_msvB; sp.tjb = db->d_tjb; sp.order = db->d_order;
@@ -292,7 +285,7 @@ static int run_stage1(ckm_engine *e, const SearchKnobs &k, const ckm_models *m, 
                                 s1.cand.as<int2>(), e->d_counters + CTR_CAND, s1.cand_cap, st))) return rc;
     e->stats.kernel_launches++;
   }
-  CKM_CUDA(cudaEventRecord(e->ev[EV_MSV], st));
+  CKM_TRY(ev_record(e, EV_MSV));
   // exact MSV on the candidates
   MsvParams p{};
   p.res = db->d_res; p.off = db->d_off; p.len = db->d_len; p.nullsc = db->d_nullsc; p.tjb = db->d_tjb;
@@ -305,7 +298,7 @@ static int run_stage1(ckm_engine *e, const SearchKnobs &k, const ckm_models *m, 
   p.use_blk = k.blk ? 1 : 0;
   if ((rc = per_class(e, p, launch_msv2, 16, launch_msv_exact, 4))) return rc;
   e->stats.kernel_launches += 1 + (p.use_blk ? N_BLK_CLASSES : 0);
-  CKM_CUDA(cudaEventRecord(e->ev[EV_BIAS], st));
+  CKM_TRY(ev_record(e, EV_BIAS));
   return CKM_OK;
 }
 
@@ -320,7 +313,7 @@ static int run_viterbi(ckm_engine *e, const ckm_models *m, FilterParams &p, bool
     const int nm = (int)m->models.size();
     const size_t nchunks = (size_t)p.in_cap / VITP_CHUNK + nm + 1;           // every model's last chunk may be partial
     const size_t words = 4 * (size_t)nm + 16 + ((size_t)p.in_cap + 1) / 2 * 2;
-    if ((rc = grp.alloc(sizeof(int32_t) * words + sizeof(int2) * nchunks))) return rc;
+    CKM_TRY(grp.alloc(sizeof(int32_t) * words + sizeof(int2) * nchunks));
     int32_t *ws = grp.as<int32_t>();
     p.vit_cls_chunks = ws + 4 * (size_t)nm;
     p.vit_idx = p.vit_cls_chunks + 16;
@@ -344,9 +337,9 @@ static int run_stage2(ckm_engine *e, const SearchKnobs &k, const ckm_models *m, 
   cudaStream_t st = e->stream;
   int rc;
   s2.cap = s1.pass_cap;
-  if ((rc = s2.a.alloc(sizeof(Candidate) * (size_t)s2.cap))) return rc;
-  if ((rc = s2.b.alloc(sizeof(Candidate) * (size_t)s2.cap))) return rc;
-  if ((rc = s2.redo.alloc(sizeof(Candidate) * (size_t)s2.cap))) return rc;
+  CKM_TRY(s2.a.alloc(sizeof(Candidate) * (size_t)s2.cap));
+  CKM_TRY(s2.b.alloc(sizeof(Candidate) * (size_t)s2.cap));
+  CKM_TRY(s2.redo.alloc(sizeof(Candidate) * (size_t)s2.cap));
   const int nsm = e->prop.multiProcessorCount;
   FilterParams p = filter_params(m, db, am);
   p.redo = s2.redo.as<Candidate>(); p.redo_count = e->d_counters + CTR_VREDO; p.redo_cap = s2.cap;
@@ -356,18 +349,18 @@ static int run_stage2(ckm_engine *e, const SearchKnobs &k, const ckm_models *m, 
   p.in = s1.pass.as<Candidate>(); p.in_count = e->d_counters + CTR_MSV; p.in_cap = s1.pass_cap;
   p.out = s2.a.as<Candidate>(); p.out_count = e->d_counters + CTR_BIAS; p.out_cap = s2.cap;
   if ((rc = launch_bias(p, nsm * 8, st))) return rc;
-  CKM_CUDA(cudaEventRecord(e->ev[EV_VIT], st));
+  CKM_TRY(ev_record(e, EV_VIT));
   // viterbi: a -> b
   p.in = s2.a.as<Candidate>(); p.in_count = e->d_counters + CTR_BIAS; p.in_cap = s2.cap;
   p.out = s2.b.as<Candidate>(); p.out_count = e->d_counters + CTR_VIT; p.out_cap = s2.cap;
   if ((rc = run_viterbi(e, m, p, k.vitp, s2.vgrp))) return rc;
-  CKM_CUDA(cudaEventRecord(e->ev[EV_FWD], st));
+  CKM_TRY(ev_record(e, EV_FWD));
   // forward: b -> a
   p.in = s2.b.as<Candidate>(); p.in_count = e->d_counters + CTR_VIT; p.in_cap = s2.cap;
   p.out = s2.a.as<Candidate>(); p.out_count = e->d_counters + CTR_FWD; p.out_cap = s2.cap;
   // widest classes first: their one-warp-per-pair kernels are the long pole of the stage, the narrow ones fill in around them
   if ((rc = per_class(e, p, launch_fwd2, 8, launch_fwd, 4, /*widest_first=*/true))) return rc;
-  CKM_CUDA(cudaEventRecord(e->ev[EV_CASCADE_END], st));
+  CKM_TRY(ev_record(e, EV_CASCADE_END));
   e->stats.kernel_launches += 3 + (k.vitp ? N_BLK_CLASSES : 0) + (p.use_blk ? 2 * N_BLK_CLASSES : 0);
   return CKM_OK;
 }
@@ -395,7 +388,8 @@ static int run_envelope_waves(ckm_engine *e, const ckm_models *m, const std::vec
     ecls[i] = (int8_t)cls_of(m->models[pw.model].M, p.use_blk != 0);
   }
   budget = std::max<int64_t>(budget, *std::max_element(need.begin(), need.end()));
-  if ((rc = d_ev.alloc(sizeof(Envelope) * ev.size())) || (rc = d_ord.alloc(sizeof(int32_t) * ev.size()))) return rc;
+  CKM_TRY(d_ev.alloc(sizeof(Envelope) * ev.size()));
+  CKM_TRY(d_ord.alloc(sizeof(int32_t) * ev.size()));
   std::vector<int32_t> eorder(ev.size());
   for (size_t w0 = 0, w1; w0 < ev.size(); w0 = w1) {
     int64_t tot = 0;
@@ -404,13 +398,13 @@ static int run_envelope_waves(ckm_engine *e, const ckm_models *m, const std::vec
     // this wave's envelopes grouped by class, largest first; one stream per class
     for (size_t i = w0; i < w1; ++i) eorder[i] = (int32_t)i;
     std::stable_sort(eorder.begin() + w0, eorder.begin() + w1, [&](int32_t a, int32_t b) { return ecls[a] != ecls[b] ? ecls[a] > ecls[b] : need[a] > need[b]; });
-    CKM_CUDA(cudaMemcpyAsync(d_ev.as<Envelope>() + w0, ev.data() + w0, sizeof(Envelope) * (w1 - w0), cudaMemcpyHostToDevice, st));
-    CKM_CUDA(cudaMemcpyAsync(d_ord.as<int32_t>() + w0, eorder.data() + w0, sizeof(int32_t) * (w1 - w0), cudaMemcpyHostToDevice, st));
+    CKM_TRY(copy_in(d_ev.as<Envelope>() + w0, ev.data() + w0, w1 - w0, st));
+    CKM_TRY(copy_in(d_ord.as<int32_t>() + w0, eorder.data() + w0, w1 - w0, st));
     p.envs = d_ev.as<Envelope>(); p.env_order = d_ord.as<int32_t>(); p.scratch = scratch.as<float>();
     if ((rc = launch_class_runs(e, eorder, ecls, w0, w1, [&](int c, int32_t b0, int32_t b1, int grid, cudaStream_t s) -> int {
           p.env_begin = b0; p.env_end = b1; return c < N_BLK_CLASSES ? launch_envelopes2(p, c, grid, s) : launch_envelopes(p, grid, s); }))) return rc;
-    CKM_CUDA(cudaStreamSynchronize(st));          // the two copies above have read the host vectors
-    if (w1 < ev.size() || !leave_last) { if ((rc = fan_in(e))) return rc; CKM_CUDA(cudaStreamSynchronize(st)); }
+    CKM_TRY(stream_sync(st));          // the two copies above have read the host vectors
+    if (w1 < ev.size() || !leave_last) { CKM_TRY(fan_in(e)); CKM_TRY(stream_sync(st)); }
   }
   return CKM_OK;
 }
@@ -448,9 +442,9 @@ static int run_cascade(ckm_engine *e, const SearchKnobs &k, const ckm_models *m,
     if (attempt > 0) e->stats.n_queue_retries++;
     if ((rc = run_stage1(e, k, m, db, am, std::max<int64_t>(n_pairs, 1), s1, nullptr, attempt))) return rc;
     if ((rc = run_stage2(e, k, m, db, am, s1, s2, nullptr, nullptr, nullptr, nullptr))) return rc;
-    CKM_CUDA(cudaMemcpyAsync(ctr, e->d_counters, sizeof(int32_t) * CTR_N, cudaMemcpyDeviceToHost, st));
-    CKM_CUDA(cudaMemcpyAsync(&cells, s1.cells.p, sizeof(cells), cudaMemcpyDeviceToHost, st));
-    CKM_CUDA(cudaStreamSynchronize(st));
+    CKM_TRY(copy_out(ctr, e->d_counters, CTR_N, st));
+    CKM_TRY(s1.cells.get(&cells, 1, st));
+    CKM_TRY(stream_sync(st));
     const bool over = ctr[CTR_CAND] > s1.cand_cap || ctr[CTR_MSV] > s1.pass_cap || ctr[CTR_BIAS] > s2.cap || ctr[CTR_VIT] > s2.cap || ctr[CTR_FWD] > s2.cap ||
                       ctr[CTR_VREDO] > s2.cap;
     if (!over) { fill_filter_stats(e, n_pairs, ctr, cells, 5); return CKM_OK; }
@@ -487,15 +481,15 @@ struct DomainStage {
 static int run_regions(ckm_engine *e, const SearchKnobs &k, const ckm_models *m, const ckm_seqdb *db, const std::vector<PairWork> &pairs, int64_t rows, DomainStage &D, Trace &tr) {
   cudaStream_t st = e->stream;
   const int npairs = (int)pairs.size();
-  const size_t rws = (size_t)std::max<int64_t>(rows, 1);
-  int rc;
-  if ((rc = D.dpairs.alloc(sizeof(PairWork) * pairs.size())) || (rc = D.dxf.alloc(sizeof(float) * rws * X_NX_HOST)) || (rc = D.dxb.alloc(sizeof(float) * rws * X_NX_HOST)) ||
-      (rc = D.dvec.alloc(sizeof(float) * rws * 4)) || (rc = D.dtbl.alloc(sizeof(float) * 16000))) return rc;
+  const size_t rws = (size_t)rows;
+  CKM_TRY(D.dpairs.put(pairs.data(), pairs.size(), st));
+  CKM_TRY(D.dxf.alloc(sizeof(float) * rws * X_NX_HOST));
+  CKM_TRY(D.dxb.alloc(sizeof(float) * rws * X_NX_HOST));
+  CKM_TRY(D.dvec.alloc(sizeof(float) * rws * 4));
+  CKM_TRY(D.dtbl.put(logsum_table().data(), 16000, st));
   const int region_cap = npairs * 8 + 1024;
-  if ((rc = D.dregions.alloc(sizeof(Region) * (size_t)region_cap))) return rc;
-  CKM_CUDA(cudaMemcpyAsync(D.dpairs.p, pairs.data(), sizeof(PairWork) * pairs.size(), cudaMemcpyHostToDevice, st));
-  CKM_CUDA(cudaMemcpyAsync(D.dtbl.p, logsum_table().data(), sizeof(float) * 16000, cudaMemcpyHostToDevice, st));
-  CKM_CUDA(cudaMemsetAsync(e->d_counters + CTR_ENV, 0, sizeof(int32_t), st));
+  CKM_TRY(D.dregions.alloc(sizeof(Region) * (size_t)region_cap));
+  CKM_TRY(set_bytes(e->d_counters + CTR_ENV, 0, sizeof(int32_t), st));
   DomdefParams &p = D.p = domdef_params(m, db, k);
   p.pairs = D.dpairs.as<PairWork>(); p.npairs = npairs;
   p.xf = D.dxf.as<float>(); p.xb = D.dxb.as<float>();
@@ -507,15 +501,14 @@ static int run_regions(ckm_engine *e, const SearchKnobs &k, const ckm_models *m,
   std::vector<int8_t> pcls((size_t)npairs);
   for (int i = 0; i < npairs; ++i) { order[i] = i; pcls[i] = (int8_t)cls_of(m->models[pairs[i].model].M, p.use_blk != 0); }
   std::stable_sort(order.begin(), order.end(), [&](int32_t a, int32_t b) { return pcls[a] != pcls[b] ? pcls[a] > pcls[b] : pairs[a].L > pairs[b].L; });
-  if ((rc = D.dporder.alloc(sizeof(int32_t) * order.size()))) return rc;
-  CKM_CUDA(cudaMemcpyAsync(D.dporder.p, order.data(), sizeof(int32_t) * order.size(), cudaMemcpyHostToDevice, st));
+  CKM_TRY(D.dporder.put(order.data(), order.size(), st));
   p.pair_order = D.dporder.as<int32_t>();
-  if ((rc = launch_class_runs(e, order, pcls, 0, (size_t)npairs, [&](int c, int32_t b0, int32_t b1, int grid, cudaStream_t s) -> int {
-        p.pair_begin = b0; p.pair_end = b1; return c < N_BLK_CLASSES ? launch_regions2(p, c, grid, s) : launch_regions(p, grid, s); }))) return rc;
-  if ((rc = fan_in(e))) return rc;
+  CKM_TRY(launch_class_runs(e, order, pcls, 0, (size_t)npairs, [&](int c, int32_t b0, int32_t b1, int grid, cudaStream_t s) -> int {
+        p.pair_begin = b0; p.pair_end = b1; return c < N_BLK_CLASSES ? launch_regions2(p, c, grid, s) : launch_regions(p, grid, s); }));
+  CKM_TRY(fan_in(e));
   int32_t nreg = 0;
-  CKM_CUDA(cudaMemcpyAsync(&nreg, e->d_counters + CTR_ENV, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-  CKM_CUDA(cudaStreamSynchronize(st));     // also the end of the copy that reads `order`
+  CKM_TRY(copy_out(&nreg, e->d_counters + CTR_ENV, 1, st));
+  CKM_TRY(stream_sync(st));     // also the end of the copy that reads `order`
   tr.mark("regions kernels");
   if (nreg > region_cap) { set_error("region queue overflow"); return CKM_ECAPACITY; }
   D.regs.resize((size_t)nreg);
@@ -554,9 +547,9 @@ static int domain_pass(ckm_engine *e, const SearchKnobs &k, const ckm_models *m,
   }
   D.doms.assign((size_t)nslots, DomainOut{});
   if (nslots == 0) return CKM_OK;
-  if ((rc = D.ddoms.alloc(sizeof(DomainOut) * (size_t)nslots)) || (rc = D.dhits.alloc(sizeof(HitOut) * pairs.size()))) return rc;
-  CKM_CUDA(cudaMemsetAsync(D.ddoms.p, 0, sizeof(DomainOut) * (size_t)nslots, st));
-  CKM_CUDA(cudaMemcpyAsync(D.dpairs.p, pairs.data(), sizeof(PairWork) * pairs.size(), cudaMemcpyHostToDevice, st));
+  CKM_TRY(D.ddoms.fill(sizeof(DomainOut) * (size_t)nslots, 0, st));
+  CKM_TRY(D.dhits.alloc(sizeof(HitOut) * pairs.size()));
+  CKM_TRY(copy_in(D.dpairs.as<PairWork>(), pairs.data(), pairs.size(), st));
   p.doms = D.ddoms.as<DomainOut>();
   // The trace ensemble of the multi-domain regions (one warp per region, latency-bound, its own stream) runs next to the
   // envelope kernels of the single-domain regions (class streams).  Next to them its dependent loads take 2-3x longer than
@@ -584,7 +577,7 @@ static int domain_pass(ckm_engine *e, const SearchKnobs &k, const ckm_models *m,
   tr.mark("envelope batch 1 launched");
   if (multi) {
     if (!ens_first && (rc = launch_ensemble())) return rc;
-    if (!envs1.empty()) { if ((rc = fan_in(e))) return rc; CKM_CUDA(cudaStreamSynchronize(st)); }
+    if (!envs1.empty()) { CKM_TRY(fan_in(e)); CKM_TRY(stream_sync(st)); }
     std::vector<std::vector<Envelope>> multi_envs; std::vector<EnsembleCaps> grow;
     int n_over = 0;
     if ((rc = ensembles_collect(ens.release(), e->aux, multi_envs, grow, &n_over))) return rc;
@@ -604,10 +597,9 @@ static int domain_pass(ckm_engine *e, const SearchKnobs &k, const ckm_models *m,
   p.hits = D.dhits.as<HitOut>();
   if ((rc = launch_scores(p, ((int)pairs.size() + 127) / 128, st))) return rc;
   e->stats.kernel_launches++;
-  CKM_CUDA(cudaMemcpyAsync(D.doms.data(), D.ddoms.p, sizeof(DomainOut) * D.doms.size(), cudaMemcpyDeviceToHost, st));
-  CKM_CUDA(cudaMemcpyAsync(D.hout.data(), D.dhits.p, sizeof(HitOut) * D.hout.size(), cudaMemcpyDeviceToHost, st));
-  CKM_CUDA(cudaStreamSynchronize(st));
-  return CKM_OK;
+  CKM_TRY(D.ddoms.get(D.doms.data(), D.doms.size(), st));
+  CKM_TRY(D.dhits.get(D.hout.data(), D.hout.size(), st));
+  return stream_sync(st);
 }
 // The domain phase: envelopes, domains and scores of every pair, repeated while a multi-domain region outgrows its capacities.
 constexpr int DOMAIN_PASSES = 4;
@@ -685,35 +677,34 @@ static std::vector<ckm_hit> assemble_rows(ckm_engine *e, const ckm_models *m, co
 
 static int do_search(ckm_engine *e, const SearchKnobs &k, const ckm_models *m, const int32_t *model_idx, int32_t nmodels,
                      const int64_t *bin_model_offsets, const ckm_seqdb *db, double Ecut, double domEcut, ckm_hit **hits_out, int64_t *nhits_out) {
-  cudaStream_t st = e->stream;
   *hits_out = nullptr; *nhits_out = 0;
-  PoolScope pool_scope(e);
+  const DeviceScope ws(e);
   QueryPlan q;
-  int rc = plan_queries(m, db, model_idx, nmodels, bin_model_offsets, q, st);
+  int rc = plan_queries(m, db, model_idx, nmodels, bin_model_offsets, q, ws.st);
   if (rc) return rc;
   std::memset(&e->stats, 0, sizeof(e->stats));
   if (q.n_pairs > ((int64_t)1 << 40)) { set_error("ckm_search: more than 2^40 (ORF x HMM) pairs in one call; search fewer bins per call"); return CKM_ECAPACITY; }
-  CKM_CUDA(cudaEventRecord(e->ev[EV_CALL], st));
+  CKM_TRY(ev_record(e, EV_CALL));
   Trace tr(k.trace);
   Stage1 s1; Stage2 s2; int32_t ctr[CTR_N];
   if ((rc = run_cascade(e, k, m, db, q.am, q.n_pairs, s1, s2, ctr))) return rc;
   tr.mark("filters done");
   std::vector<PairWork> pairs; int64_t rows = 0;
   if ((rc = sorted_pairs(db, s2.a.as<Candidate>(), ctr[CTR_FWD], pairs, rows))) return rc;
-  CKM_CUDA(cudaEventRecord(e->ev[EV_DOMDEF], st));
+  CKM_TRY(ev_record(e, EV_DOMDEF));
   tr.mark("pair list sorted");
   DomainStage D;
   if (!pairs.empty()) {
     if ((rc = run_regions(e, k, m, db, pairs, rows, D, tr))) return rc;
     if ((rc = run_domain_phase(e, k, m, pairs, D, tr))) return rc;
   }
-  CKM_CUDA(cudaEventRecord(e->ev[EV_END], st));
+  CKM_TRY(ev_record(e, EV_END));
   CKM_CUDA(cudaEventSynchronize(e->ev[EV_END]));
   tr.mark("scores + downloads");
   const std::vector<ckm_hit> rows_out = assemble_rows(e, m, db, q, pairs, D.hout, D.doms, Ecut, domEcut);
   tr.mark("rows assembled");
-  cudaEventElapsedTime(&e->stats.ms_domdef, e->ev[EV_DOMDEF], e->ev[EV_END]);
-  cudaEventElapsedTime(&e->stats.ms_total, e->ev[EV_CALL], e->ev[EV_END]);
+  ev_elapsed(e, &e->stats.ms_domdef, EV_DOMDEF, EV_END);
+  ev_elapsed(e, &e->stats.ms_total, EV_CALL, EV_END);
   if (!rows_out.empty()) {
     ckm_hit *out = (ckm_hit *)std::malloc(sizeof(ckm_hit) * rows_out.size());
     if (!out) { set_error("out of host memory"); return CKM_ENOMEM; }
@@ -731,28 +722,23 @@ static int do_search(ckm_engine *e, const SearchKnobs &k, const ckm_models *m, c
 // best-scoring domain as the search pipeline defines it, the rest of it being flank.
 static int align_pass(ckm_engine *e, const SearchKnobs &k, const ckm_models *m, const ckm_seqdb *db, std::vector<PairWork> &pairs,
                       std::vector<Envelope> &envs, int64_t rows, std::vector<int32_t> &trace, std::vector<DomainOut> &doms) {
-  cudaStream_t st = e->stream;
-  PoolScope pool_scope(e);
+  const DeviceScope ws(e);
   DevBuf dpairs, dn2, dtrace, ddoms, dscratch, denvs, deorder;
-  int rc;
   const size_t rws = (size_t)rows;
-  if ((rc = dpairs.alloc(sizeof(PairWork) * pairs.size())) || (rc = dn2.alloc(sizeof(float) * rws)) || (rc = dtrace.alloc(sizeof(int32_t) * rws)) ||
-      (rc = ddoms.alloc(sizeof(DomainOut) * pairs.size()))) return rc;
-  CKM_CUDA(cudaMemcpyAsync(dpairs.p, pairs.data(), sizeof(PairWork) * pairs.size(), cudaMemcpyHostToDevice, st));
-  CKM_CUDA(cudaMemsetAsync(dn2.p, 0, sizeof(float) * rws, st));
-  CKM_CUDA(cudaMemsetAsync(dtrace.p, 0, sizeof(int32_t) * rws, st));
-  CKM_CUDA(cudaMemsetAsync(ddoms.p, 0, sizeof(DomainOut) * pairs.size(), st));
+  CKM_TRY(dpairs.put(pairs.data(), pairs.size(), ws.st));
+  CKM_TRY(dn2.fill(sizeof(float) * rws, 0, ws.st));
+  CKM_TRY(dtrace.fill(sizeof(int32_t) * rws, 0, ws.st));
+  CKM_TRY(ddoms.fill(sizeof(DomainOut) * pairs.size(), 0, ws.st));
   DomdefParams p = domdef_params(m, db, k);
   p.pairs = dpairs.as<PairWork>(); p.npairs = (int32_t)pairs.size();
   p.n2sc = dn2.as<float>(); p.trace = dtrace.as<int32_t>();
   p.doms = ddoms.as<DomainOut>();
-  if ((rc = run_envelope_waves(e, m, pairs, p, k.env_budget, dscratch, envs, denvs, deorder, false))) return rc;
+  CKM_TRY(run_envelope_waves(e, m, pairs, p, k.env_budget, dscratch, envs, denvs, deorder, false));
   trace.resize(rws);
   doms.resize(pairs.size());
-  CKM_CUDA(cudaMemcpyAsync(trace.data(), dtrace.p, sizeof(int32_t) * rws, cudaMemcpyDeviceToHost, st));
-  CKM_CUDA(cudaMemcpyAsync(doms.data(), ddoms.p, sizeof(DomainOut) * doms.size(), cudaMemcpyDeviceToHost, st));
-  CKM_CUDA(cudaStreamSynchronize(st));
-  return CKM_OK;
+  CKM_TRY(dtrace.get(trace.data(), rws, ws.st));
+  CKM_TRY(ddoms.get(doms.data(), doms.size(), ws.st));
+  return stream_sync(ws.st);
 }
 
 // The group driver behind ckm_align and ckm_align_groups: the sequences of group g against model group_model[g], every group
@@ -903,31 +889,28 @@ int ckm_write_domtblout(const ckm_models *m, const ckm_hit *hits, int64_t nhits,
 int ckm_filter_scores(ckm_engine *e, const ckm_models *m, const int32_t *model_idx, int32_t nmodels,
                       const ckm_seqdb *db, float *filtersc_out, float *vit_out, float *fwd_out, uint8_t *passed_out) {
   if (!e || !m || !db || !filtersc_out || !vit_out || !fwd_out || !passed_out) { set_error("ckm_filter_scores: bad argument"); return CKM_EINVAL; }
-  cudaSetDevice(e->device);
   const SearchKnobs k = read_knobs(false);
-  PoolScope pool_scope(e);
+  const DeviceScope ws(e);
   QueryPlan q;
-  int rc = plan_queries(m, db, model_idx, nmodels, nullptr, q, e->stream);
+  int rc = plan_queries(m, db, model_idx, nmodels, nullptr, q, ws.st);
   if (rc) return rc;
   const int64_t n = q.n_pairs;
   DevBuf dfs, dvit, dfwd, dpass;
-  const size_t nf = (size_t)std::max<int64_t>(n, 1);
-  if ((rc = dfs.alloc(sizeof(float) * nf)) || (rc = dvit.alloc(sizeof(float) * nf)) || (rc = dfwd.alloc(sizeof(float) * nf)) ||
-      (rc = dpass.alloc(nf + 4))) return rc;
+  const size_t nf = (size_t)n;
   // NaN-fill the float outputs, zero the flags
-  for (DevBuf *b : {&dfs, &dvit, &dfwd}) CKM_CUDA(cudaMemsetAsync(b->p, 0xff, sizeof(float) * nf, e->stream));
-  CKM_CUDA(cudaMemsetAsync(dpass.p, 0, nf + 4, e->stream));
+  for (DevBuf *b : {&dfs, &dvit, &dfwd}) CKM_TRY(b->fill(sizeof(float) * nf, 0xff, ws.st));
+  CKM_TRY(dpass.fill(nf + 4, 0, ws.st));
   Stage1 s1; Stage2 s2;
   std::memset(&e->stats, 0, sizeof(e->stats));
   if ((rc = run_stage1(e, k, m, db, q.am, n, s1, nullptr))) return rc;
   if ((rc = run_stage2(e, k, m, db, q.am, s1, s2, dfs.as<float>(), dvit.as<float>(), dfwd.as<float>(), dpass.as<uint8_t>()))) return rc;
   int32_t ctr[CTR_N];
-  CKM_CUDA(cudaMemcpyAsync(ctr, e->d_counters, sizeof(ctr), cudaMemcpyDeviceToHost, e->stream));
-  CKM_CUDA(cudaMemcpyAsync(filtersc_out, dfs.p, sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost, e->stream));
-  CKM_CUDA(cudaMemcpyAsync(vit_out, dvit.p, sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost, e->stream));
-  CKM_CUDA(cudaMemcpyAsync(fwd_out, dfwd.p, sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost, e->stream));
-  CKM_CUDA(cudaMemcpyAsync(passed_out, dpass.p, (size_t)n, cudaMemcpyDeviceToHost, e->stream));
-  CKM_CUDA(cudaStreamSynchronize(e->stream));
+  CKM_TRY(copy_out(ctr, e->d_counters, CTR_N, ws.st));
+  CKM_TRY(dfs.get(filtersc_out, nf, ws.st));
+  CKM_TRY(dvit.get(vit_out, nf, ws.st));
+  CKM_TRY(dfwd.get(fwd_out, nf, ws.st));
+  CKM_TRY(dpass.get(passed_out, nf, ws.st));
+  CKM_TRY(stream_sync(ws.st));
   if (ctr[CTR_CAND] > s1.cand_cap || ctr[CTR_MSV] > s1.pass_cap) { set_error("candidate queue overflow"); return CKM_ECAPACITY; }
   // MSV pass flags come from the stage-1 pass list
   std::vector<Candidate> pass1((size_t)ctr[CTR_MSV]);
@@ -940,25 +923,25 @@ int ckm_filter_scores(ckm_engine *e, const ckm_models *m, const int32_t *model_i
 int ckm_viterbi_scores(ckm_engine *e, const ckm_models *m, const int32_t *model_idx, int32_t nmodels,
                        const ckm_seqdb *db, int32_t mode, float *vit_out) {
   if (!e || !m || !db || !vit_out) { set_error("ckm_viterbi_scores: bad argument"); return CKM_EINVAL; }
-  cudaSetDevice(e->device);
-  cudaStream_t st = e->stream;
+  const DeviceScope ws(e);
+  const cudaStream_t st = ws.st;
   const int ndb = (int)m->models.size();
   if (model_idx == nullptr) nmodels = ndb;
   const int64_t n = (int64_t)nmodels * db->nseq;
   if (n > ((int64_t)1 << 30)) { set_error("ckm_viterbi_scores: too many pairs for one call"); return CKM_ECAPACITY; }
-  PoolScope pool_scope(e);
   ActiveMasks am; std::vector<int32_t> slot;
   int rc = build_masks(m, db, model_idx, nmodels, nullptr, am, slot, st);
   if (rc) return rc;
   std::vector<int32_t> slot_model((size_t)std::max(nmodels, 1));
   for (int i = 0; i < nmodels; ++i) slot_model[i] = model_idx ? model_idx[i] : i;
-  const size_t nf = (size_t)std::max<int64_t>(n, 1);
+  const size_t nf = (size_t)n;
   DevBuf dsm, din, dout, dredo, dvit, dgrp;
-  if ((rc = dsm.alloc(sizeof(int32_t) * slot_model.size())) || (rc = din.alloc(sizeof(Candidate) * nf)) || (rc = dout.alloc(sizeof(Candidate) * nf)) ||
-      (rc = dredo.alloc(sizeof(Candidate) * nf)) || (rc = dvit.alloc(sizeof(float) * nf))) return rc;
-  CKM_CUDA(cudaMemcpyAsync(dsm.p, slot_model.data(), sizeof(int32_t) * slot_model.size(), cudaMemcpyHostToDevice, st));
-  CKM_CUDA(cudaMemsetAsync(e->d_counters, 0, CTR_N * sizeof(int32_t), st));
-  CKM_CUDA(cudaMemsetAsync(dvit.p, 0xff, sizeof(float) * nf, st));
+  CKM_TRY(dsm.put(slot_model.data(), slot_model.size(), st));
+  CKM_TRY(din.alloc(sizeof(Candidate) * nf));
+  CKM_TRY(dout.alloc(sizeof(Candidate) * nf));
+  CKM_TRY(dredo.alloc(sizeof(Candidate) * nf));
+  CKM_TRY(set_bytes(e->d_counters, 0, CTR_N * sizeof(int32_t), st));
+  CKM_TRY(dvit.fill(sizeof(float) * nf, 0xff, st));
   std::memset(&e->stats, 0, sizeof(e->stats));
   if (n > 0) {
     if ((rc = launch_all_pairs(din.as<Candidate>(), e->d_counters + CTR_BIAS, dsm.as<int32_t>(), nmodels, db->nseq, st))) return rc;
@@ -971,9 +954,9 @@ int ckm_viterbi_scores(ckm_engine *e, const ckm_models *m, const int32_t *model_
     if ((rc = run_viterbi(e, m, p, mode == 0, dgrp))) return rc;
   }
   int32_t ctr[CTR_N];
-  CKM_CUDA(cudaMemcpyAsync(ctr, e->d_counters, sizeof(ctr), cudaMemcpyDeviceToHost, st));
-  CKM_CUDA(cudaMemcpyAsync(vit_out, dvit.p, sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost, st));
-  CKM_CUDA(cudaStreamSynchronize(st));
+  CKM_TRY(copy_out(ctr, e->d_counters, CTR_N, st));
+  CKM_TRY(dvit.get(vit_out, nf, st));
+  CKM_TRY(stream_sync(st));
   e->stats.n_pairs = n; e->stats.n_past_bias = ctr[CTR_BIAS]; e->stats.n_past_vit = ctr[CTR_VIT]; e->stats.n_vit_redo = ctr[CTR_VREDO];
   return CKM_OK;
 }
@@ -981,25 +964,23 @@ int ckm_viterbi_scores(ckm_engine *e, const ckm_models *m, const int32_t *model_
 int ckm_msv_scores(ckm_engine *e, const ckm_models *m, const int32_t *model_idx, int32_t nmodels,
                    const ckm_seqdb *db, int32_t *xj_out) {
   if (!e || !m || !db || !xj_out) { set_error("ckm_msv_scores: bad argument"); return CKM_EINVAL; }
-  cudaSetDevice(e->device);
   const SearchKnobs k = read_knobs(false);
-  PoolScope pool_scope(e);
+  const DeviceScope ws(e);
   QueryPlan q;
-  int rc = plan_queries(m, db, model_idx, nmodels, nullptr, q, e->stream);
+  int rc = plan_queries(m, db, model_idx, nmodels, nullptr, q, ws.st);
   if (rc) return rc;
   const int64_t n = q.n_pairs;
   DevBuf dense;
-  if ((rc = dense.alloc(sizeof(int32_t) * (size_t)std::max<int64_t>(n, 1)))) return rc;
-  CKM_CUDA(cudaMemsetAsync(dense.p, 0xff, sizeof(int32_t) * (size_t)n, e->stream));
+  CKM_TRY(dense.fill(sizeof(int32_t) * (size_t)n, 0xff, ws.st));
   Stage1 s1;
   std::memset(&e->stats, 0, sizeof(e->stats));
   if ((rc = run_stage1(e, k, m, db, q.am, n, s1, dense.as<int32_t>()))) return rc;
   int32_t ctr[CTR_N];
-  CKM_CUDA(cudaMemcpyAsync(ctr, e->d_counters, sizeof(ctr), cudaMemcpyDeviceToHost, e->stream));
+  CKM_TRY(copy_out(ctr, e->d_counters, CTR_N, ws.st));
   unsigned long long cells = 0;
-  CKM_CUDA(cudaMemcpyAsync(&cells, s1.cells.p, sizeof(cells), cudaMemcpyDeviceToHost, e->stream));
-  CKM_CUDA(cudaMemcpyAsync(xj_out, dense.p, sizeof(int32_t) * (size_t)n, cudaMemcpyDeviceToHost, e->stream));
-  CKM_CUDA(cudaStreamSynchronize(e->stream));
+  CKM_TRY(s1.cells.get(&cells, 1, ws.st));
+  CKM_TRY(dense.get(xj_out, (size_t)n, ws.st));
+  CKM_TRY(stream_sync(ws.st));
   if (ctr[CTR_CAND] > s1.cand_cap || ctr[CTR_MSV] > s1.pass_cap) { set_error("candidate queue overflow"); return CKM_ECAPACITY; }
   fill_filter_stats(e, n, ctr, cells, 2);     // stage 1 only: the later counters are still zero
   return CKM_OK;

@@ -243,29 +243,21 @@ int ckm_window_stats(ckm_engine *e, const uint8_t *bytes, int64_t nbytes, const 
   const int64_t nwin = win_off[nseq];
   if (nwin == 0) return CKM_OK;
   if (!acgt_out) { set_error("ckm_window_stats: bad argument"); return CKM_EINVAL; }
-  cudaSetDevice(e->device);
-  PoolScope pool_scope(e);
-  cudaStream_t st = e->stream;
+  const DeviceScope ws(e);
   const int dyn_smem = WN_WARPS * WN_WARP_SMEM;
   NtUpload u;
-  if (int rc = nt_upload(e, "ckm_window_stats", bytes, nbytes, starts, lens, nseq, (const void *)window_scan_kernel, WN_WARPS,
-                         WN_CTAS_PER_SM, dyn_smem, u))
-    return rc;
+  CKM_TRY(nt_upload(e, "ckm_window_stats", bytes, nbytes, starts, lens, nseq, (const void *)window_scan_kernel, WN_WARPS,
+                    WN_CTAS_PER_SM, dyn_smem, u));
   std::vector<long long> seq_info((size_t)2 * nseq + 1);           // starts, then win_off
   for (int32_t s = 0; s < nseq; ++s) seq_info[s] = starts[s];
   for (int32_t s = 0; s <= nseq; ++s) seq_info[(size_t)nseq + s] = win_off[s];
   DevBuf dinfo, dacgt, dkm, dsig, dtd;
-  int rc;
-  const size_t km_bytes = bin_sig ? sizeof(uint32_t) * WN_COLS * (size_t)nwin : 0;
-  if ((rc = dinfo.alloc(sizeof(long long) * seq_info.size())) ||
-      (rc = dacgt.alloc(sizeof(int64_t) * 4 * (size_t)nwin)) ||
-      (bin_sig && ((rc = dkm.alloc(km_bytes)) || (rc = dsig.alloc(sizeof(double) * WN_COLS)) || (rc = dtd.alloc(sizeof(double) * (size_t)nwin)))))
-    return rc;
-  CKM_CUDA(cudaMemcpyAsync(dinfo.p, seq_info.data(), sizeof(long long) * seq_info.size(), cudaMemcpyHostToDevice, st));
-  CKM_CUDA(cudaMemsetAsync(dacgt.p, 0, sizeof(int64_t) * 4 * (size_t)nwin, st));
+  CKM_TRY(dinfo.put(seq_info.data(), seq_info.size(), ws.st));
+  CKM_TRY(dacgt.fill(sizeof(int64_t) * 4 * (size_t)nwin, 0, ws.st));
   if (bin_sig) {
-    CKM_CUDA(cudaMemsetAsync(dkm.p, 0, km_bytes, st));
-    CKM_CUDA(cudaMemcpyAsync(dsig.p, bin_sig, sizeof(double) * WN_COLS, cudaMemcpyHostToDevice, st));
+    CKM_TRY(dkm.fill(sizeof(uint32_t) * WN_COLS * (size_t)nwin, 0, ws.st));
+    CKM_TRY(dsig.put(bin_sig, WN_COLS, ws.st));
+    CKM_TRY(dtd.alloc(sizeof(double) * (size_t)nwin));
   }
   WinParams q;
   std::memset(&q, 0, sizeof(q));
@@ -276,20 +268,20 @@ int ckm_window_stats(ckm_engine *e, const uint8_t *bytes, int64_t nbytes, const 
     uint8_t code[WN_COLS];                                        // a column and its code's reverse complement share it
     for (int c = 0, n = km_col_codes(4, code); c < n; ++c) q.col_of[code[c]] = q.col_of[km_revcomp(code[c], 4)] = (uint8_t)c;
   }
-  CKM_CUDA(cudaEventRecord(e->ev[0], st));
+  CKM_TRY(ev_record(e, 0));
   if (u.nrows > 0) {
-    window_scan_kernel<<<u.grid, WN_THREADS, dyn_smem, st>>>(q);
+    window_scan_kernel<<<u.grid, WN_THREADS, dyn_smem, ws.st>>>(q);
     CKM_CUDA(cudaGetLastError());
   }
   if (bin_sig) {
-    window_dist_kernel<<<(unsigned)((nwin + WN_WARPS - 1) / WN_WARPS), WN_THREADS, 0, st>>>(dkm.as<uint32_t>(), nwin, dsig.as<double>(), dtd.as<double>());
+    window_dist_kernel<<<(unsigned)((nwin + WN_WARPS - 1) / WN_WARPS), WN_THREADS, 0, ws.st>>>(dkm.as<uint32_t>(), nwin, dsig.as<double>(), dtd.as<double>());
     CKM_CUDA(cudaGetLastError());
   }
-  CKM_CUDA(cudaEventRecord(e->ev[1], st));
-  CKM_CUDA(cudaMemcpyAsync(acgt_out, dacgt.p, sizeof(int64_t) * 4 * (size_t)nwin, cudaMemcpyDeviceToHost, st));
-  if (bin_sig) CKM_CUDA(cudaMemcpyAsync(td_out, dtd.p, sizeof(double) * (size_t)nwin, cudaMemcpyDeviceToHost, st));
-  CKM_CUDA(cudaStreamSynchronize(st));
-  if (kernel_ms_out) CKM_CUDA(cudaEventElapsedTime(kernel_ms_out, e->ev[0], e->ev[1]));
+  CKM_TRY(ev_record(e, 1));
+  CKM_TRY(dacgt.get(acgt_out, 4 * (size_t)nwin, ws.st));
+  if (bin_sig) CKM_TRY(dtd.get(td_out, (size_t)nwin, ws.st));
+  CKM_TRY(stream_sync(ws.st));
+  CKM_TRY(ev_elapsed(e, kernel_ms_out, 0, 1));
   return CKM_OK;
 }
 
