@@ -89,7 +89,7 @@ SYMBOLS = ["ckm_init", "ckm_destroy", "ckm_last_error", "ckm_version", "ckm_devi
            "ckm_kmer_counts", "ckm_kmer_columns", "ckm_format_kmer_profiles", "ckm_merge_pairs", "ckm_format_merger_rows",
            "ckm_bgzf_blocks", "ckm_bgzf_inflate", "ckm_bam_coverage", "ckm_bam_windows",
            "ckm_parse_kmer_profiles", "ckm_sigs_create", "ckm_sigs_free", "ckm_outlier_scores", "ckm_window_stats",
-           "ckm_id_join", "ckm_format_unbinned"]
+           "ckm_id_join", "ckm_format_unbinned", "ckm_length_profile"]
 
 _lib = None
 
@@ -135,6 +135,7 @@ def lib():
                               C.POINTER(C.c_float)]
     L.ckm_format_unbinned.argtypes = [vp, vp, vp, vp, vp, vp, vp, i64, vp, i64, vp, i64, C.POINTER(i64), C.POINTER(i64)]
     L.ckm_window_stats.argtypes = [vp, vp, i64, vp, vp, i32, i64, vp, vp, vp, vp, C.POINTER(C.c_float)]
+    L.ckm_length_profile.argtypes = [vp, vp, vp, i32, vp, i32, vp, vp, vp, vp, vp, vp, C.POINTER(C.c_float)]
     L.ckm_bgzf_blocks.argtypes = [vp, i64, i64, vp, i64, C.POINTER(i64), C.POINTER(i64)]
     L.ckm_bgzf_inflate.argtypes = [vp, vp, i64, i64, vp, i64, vp, i64, C.POINTER(i64), C.POINTER(C.c_float)]
     L.ckm_bam_coverage.argtypes = [vp, vp, i64, i64, vp, i64, vp, vp, i64, i32, C.POINTER(BamFilter), vp, vp, C.POINTER(i64)]

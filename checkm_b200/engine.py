@@ -369,6 +369,30 @@ class Engine:
                                           None if td is None else td.ctypes.data, C.byref(ms)))
         return acgt, td, float(ms.value)
 
+    def length_profile(self, lens, bin_off, x):
+        """The length profile of many bins in one device call (ckm_length_profile; bin b = lens[bin_off[b]:bin_off[b + 1]],
+        x ascending).  Returns per bin the total, the Nx list (nbins x len(x), -1 past the thresholds reached), the status
+        (0 OK, 1 IndexError at the record of rank fail, 2 only fail thresholds reached), fail, the 10 length-class counts
+        (nbins x 10); per record its rank in descending length order; and the kernel's duration in ms."""
+        lens = np.ascontiguousarray(lens, dtype=np.int64)
+        bin_off = np.ascontiguousarray(bin_off, dtype=np.int64)
+        x = np.ascontiguousarray(x, dtype=np.float64)
+        nbins, m = len(bin_off) - 1, len(x)
+        if nbins < 0 or int(bin_off[-1]) != len(lens):
+            raise ValueError("length_profile: bin_off must start at 0 and end at len(lens)")
+        total = np.zeros(nbins, dtype=np.int64)
+        nx = np.zeros((nbins, m), dtype=np.int64)
+        status = np.zeros(nbins, dtype=np.int32)
+        fail = np.zeros(nbins, dtype=np.int64)
+        classes = np.zeros((nbins, 10), dtype=np.int64)
+        rank = np.zeros(len(lens), dtype=np.int32)
+        ms = C.c_float()
+        check(_lib.lib().ckm_length_profile(self._h, lens.ctypes.data if lens.size else None, bin_off.ctypes.data, nbins,
+                                            x.ctypes.data if m else None, m, total.ctypes.data, nx.ctypes.data,
+                                            status.ctypes.data, fail.ctypes.data, classes.ctypes.data,
+                                            rank.ctypes.data if rank.size else None, C.byref(ms)))
+        return total, nx, status, fail, classes, rank, float(ms.value)
+
     def bgzf_inflate(self, comp, blocks, comp_base=0):
         """The payloads of BGZF `blocks` (a bam.BLOCK_DTYPE table of file offsets; comp[0] is the byte at file offset
         comp_base) inflated back to back on the device (ckm_bgzf_inflate), and the inflate kernel's duration in ms."""

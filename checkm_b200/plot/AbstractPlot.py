@@ -1,10 +1,12 @@
-"""The part of the reference's plot base class (checkm/plot/AbstractPlot.py) that the window plots use: the rcParams, the
-Figure on an Agg canvas, the axes colour and savePlot; plus the pieces the plots share -- one bin's window statistics from
-the device (`BinWindows`), the histogram edges, the "prettify" block and the lower half of the delta-vs-length panels."""
+"""The part of the reference's plot base class (checkm/plot/AbstractPlot.py) that the plots use: the rcParams, the
+Figure on an Agg canvas, the axes colour, savePlot and yLabelExtents; plus the pieces the plots share -- one bin's window
+statistics from the device (`BinWindows`), the length profiles of many bins from one device call (`length_profiles`), the
+histogram edges, the "prettify" block and the lower half of the delta-vs-length panels."""
 import logging
 import sys
 
 import matplotlib as mpl
+import matplotlib.transforms as mtransforms
 from matplotlib.backends.backend_agg import FigureCanvasAgg as FigureCanvas
 from matplotlib.figure import Figure
 
@@ -36,6 +38,17 @@ class AbstractPlot(FigureCanvas):
         imgFormat = filename[filename.rfind('.') + 1:]
         if imgFormat in ('png', 'pdf', 'ps', 'eps', 'svg'):
             self.fig.savefig(filename, format=imgFormat, dpi=dpi, facecolor='white', edgecolor='white', bbox_inches='tight')
+
+    def yLabelExtents(self, labels, fontSize, rotation=0):
+        """The bounds of the y tick labels in figure fractions, measured on a temporary axes that fills the figure."""
+        self.fig.clear()
+        tempAxes = self.fig.add_axes([0, 0, 1.0, 1.0])
+        tempAxes.set_yticks(np.arange(len(labels)))
+        yLabels = tempAxes.set_yticklabels(labels, size=fontSize, rotation=rotation)
+        bboxes = [label.get_window_extent(self.get_renderer()).transformed(self.fig.transFigure.inverted()) for label in yLabels]
+        yLabelBounds = mtransforms.Bbox.union(bboxes)
+        self.fig.clear()
+        return yLabelBounds
 
     # ---- shared by the plots ----
     def _fatal(self, message):
@@ -85,12 +98,7 @@ class BinWindows(object):
     bin's signature (BinTools.binTetraSig over `tetraSigs`), so plots that share a window size share the call."""
 
     def __init__(self, fastaFile, tetraSigs=None, sigWindowSize=None):
-        try:
-            self.ids, self.data, self.starts, self.lens = seqio.scan_nt_fasta(seqio.read_bytes(fastaFile))
-        except Exception as e:                        # util/seqUtils.py:205-209
-            print(e)
-            logging.getLogger('timestamp').error("Failed to process sequence file: {}".format(fastaFile))
-            sys.exit(1)
+        self.ids, self.data, self.starts, self.lens = read_bin(fastaFile)
         raw = self.data.tobytes()
         self.seqs = {i: raw[a:a + n].decode('latin-1') for i, a, n in zip(self.ids, self.starts.tolist(), self.lens.tolist())}
         self.binId = binIdFromFilename(fastaFile)
@@ -132,3 +140,61 @@ class BinWindows(object):
             off = self.windows(windowSize)[0]
             plot._fatal('Window %d (%d bp from position %d) of sequence %s in bin %s has no A, C, G or T: its %s is undefined.'
                         % (w - int(off[s]), windowSize, (w - int(off[s])) * windowSize, self.ids[s], self.binId, what))
+
+
+def read_bin(fastaFile):
+    """A bin as the reference's readFasta sees it (seqio.scan_nt_fasta: ids in dict order, a repeated id keeping its last
+    record); a file that cannot be read logs readFasta's error and exits with status 1."""
+    try:
+        return seqio.scan_nt_fasta(seqio.read_bytes(fastaFile))
+    except Exception as e:                            # util/seqUtils.py:205-209
+        print(e)
+        logging.getLogger('timestamp').error("Failed to process sequence file: {}".format(fastaFile))
+        sys.exit(1)
+
+
+NX_OK, NX_INDEX, NX_SHORT = 0, 1, 2                   # ckm_length_profile's status of calculateNx
+
+
+class LengthProfile(object):
+    """One bin's share of a `ckm_length_profile` call: ids and lengths (readFasta's dict order), the total, the Nx list
+    and its status (with `fail`: the rank of the record where calculateNx raises IndexError, or the number of thresholds
+    reached), the 10 length-class counts of len_hist, and every record's rank in descending length order."""
+
+    def __init__(self, binFile, ids, lens, total, nx, status, fail, classes, rank):
+        self.binFile, self.binId = binFile, binIdFromFilename(binFile)
+        self.ids, self.lens, self.total = ids, lens, total
+        self.nx, self.status, self.fail, self.classes, self.rank = nx, status, fail, classes, rank
+
+    def nxList(self):
+        """calculateNx's return value when it returns (status NX_OK or NX_SHORT), as Python ints."""
+        return self.nx[:len(self.nx) if self.status == NX_OK else self.fail].tolist()
+
+    def sequenceAtRank(self, r):
+        return self.ids[int(np.flatnonzero(self.rank == r)[0])]
+
+
+def nx_fractions(step_size):
+    """nx_plot's x: np.arange(0, 1 + step/2, step), as NxPlot.plot makes it."""
+    return np.arange(0, 1.0 + 0.5 * step_size, step_size)
+
+
+def length_profiles(binFiles, step_size=0.05, x=None):
+    """The length profiles of many bins from one device call (ckm_length_profile): each bin read once as readFasta reads
+    it, then the totals, the Nx lists at x (default: nx_fractions(step_size), sorted), the length classes and the ranks of
+    every bin together.  Returns one LengthProfile per bin file, in order."""
+    x = np.sort(nx_fractions(step_size) if x is None else np.asarray(x, dtype=np.float64))
+    if len(x) == 0:
+        raise ValueError('length_profiles: no Nx fractions')
+    bins = [read_bin(f) for f in binFiles]
+    counts = np.array([len(b[3]) for b in bins], dtype=np.int64)
+    off = np.zeros(len(bins) + 1, dtype=np.int64)
+    np.cumsum(counts, out=off[1:])
+    lens = np.concatenate([b[3] for b in bins]) if bins else np.zeros(0, dtype=np.int64)
+    try:
+        total, nx, status, fail, classes, rank, _ = runtime.engine().length_profile(lens, off, x)
+    except CkmError as e:
+        logging.getLogger('timestamp').error('Length profile of bins %s: %s' % (', '.join(binIdFromFilename(f) for f in binFiles), e))
+        sys.exit(1)
+    return [LengthProfile(f, b[0], lens[off[i]:off[i + 1]], int(total[i]), nx[i], int(status[i]), int(fail[i]), classes[i],
+                          rank[off[i]:off[i + 1]]) for i, (f, b) in enumerate(zip(binFiles, bins))]

@@ -451,6 +451,22 @@ int  ckm_format_unbinned(const char *ids, const int64_t *id_start, const int64_t
                          const int64_t *starts, const int64_t *lens, const int64_t *acgt, int64_t n, char *fasta_out,
                          int64_t fasta_cap, char *stats_out, int64_t stats_cap, int64_t *fasta_len_out, int64_t *stats_len_out);
 
+/* ---- length profiles (`checkm nx_plot`, `len_hist`, `marker_plot`; checkm/plot/nxPlot.py, lengthHistogram.py,
+ * markerGenePosPlot.py): every bin's record lengths sorted, summed and classed in one device pass (csrc/lengths.cu states
+ * the arithmetic). ---- */
+/* lens: the record lengths of every bin back to back (one per id, readFasta's dict), bin b = lens[bin_off[b] ..
+ * bin_off[b + 1]), bin_off[0] = 0.  x (m >= 1, ascending, no NaN): the Nx fractions; threshold j of bin b is x[j] * total
+ * in float64.  Per bin: total_out, the sum of its lengths; nx_out (nbins x m), calculateNx's list, -1 past the thresholds
+ * reached; status_out 0 = the reference's loop ends with m values, 1 = it raises IndexError at the record of rank
+ * fail_out[b], 2 = it reaches only fail_out[b] < m thresholds (an empty bin: 0); fail_out is -1 with status 0;
+ * class_out (nbins x 10), np.histogram of len / 1e3 over [0, 1, 2, 5, 10, 20, 50, 100, 200, 500, 1e12].  Per record:
+ * rank_out, its position in its bin's lengths sorted descending, equal lengths in record order.  A negative length, a
+ * bin total past 2^63 - 1, a bin of 2^31 records or more, or a bad x: CKM_EINVAL before any launch.  kernel_ms_out
+ * (optional): the kernel's duration by CUDA events. */
+int  ckm_length_profile(ckm_engine *e, const int64_t *lens, const int64_t *bin_off, int32_t nbins, const double *x, int32_t m,
+                        int64_t *total_out, int64_t *nx_out, int32_t *status_out, int64_t *fail_out, int64_t *class_out,
+                        int32_t *rank_out, float *kernel_ms_out);
+
 #ifdef __cplusplus
 }
 #endif
